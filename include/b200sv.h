@@ -219,11 +219,6 @@ int b200sv_phase_flip_if_less(b200sv_t s, uint64_t greater_perm, int start, int 
 int b200sv_apply_gates(b200sv_t s, int n_gates, const uint64_t* off1, const uint64_t* off2, const uint64_t* pmasks,
     const double* mats8);
 
-/* Scheduler diagnostic (no device needed): how many fused sweeps / in-tile passes a gate list would take.
- * kinds[i]: 0 real 2x2 (H-like), 1 diagonal (T/CZ-like), 2 X-like (CNOT), 3 complex general; cmasks = control qubits. */
-int b200sv_plan_dry_run(int n_qubits, int precision, int n_gates, const int* targets, const uint64_t* cmasks,
-    const int* kinds, int* n_sweeps, int* n_passes);
-
 /* Test hook (no device needed, never on the engine's path): plan + encode the gate list exactly as b200sv_apply2x2 /
  * the fused flush would, then interpret every encoded sweep program on a HOST state vector (n_qubits <= 30;
  * interleaved re/im of the given precision).  Gate i is Apply2x2(off1[i], off2[i], mats8 + 8 i, powers = bits of

@@ -7,7 +7,7 @@ import subprocess
 from ctypes import POINTER, c_char_p, c_double, c_int, c_uint64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# B200SV_LIB selects another build of the same library (tuning variants: scripts/build_variants.sh); default = the in-tree product
+# B200SV_LIB selects another build of the same library (to A/B-time two builds in one session); default = the in-tree product
 LIB_PATH = os.environ.get("B200SV_LIB") or os.path.join(_HERE, "libb200sv.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["b200sv.cu", "fused.cu"]
@@ -101,8 +101,6 @@ SIGNATURES = {
                            POINTER(c_double)],
     "b200sv_finish": [H],
     "b200sv_set_fusion": [H, c_int],
-    "b200sv_plan_dry_run": [c_int, c_int, c_int, POINTER(c_int), POINTER(c_uint64), POINTER(c_int), POINTER(c_int),
-                            POINTER(c_int)],
     "b200sv_emulate_fused": [c_int, c_int, c_int, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_double),
                              c_void_p],
     "b200sv_plan_gates": [c_int, c_int, c_int, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_double),

@@ -3513,15 +3513,6 @@ int b200sv_timer_end(b200sv_t s, double* ms)
     return B200SV_OK;
 }
 
-int b200sv_plan_dry_run(int n_qubits, int precision, int n_gates, const int* targets, const uint64_t* cmasks, const int* kinds,
-    int* n_sweeps, int* n_passes)
-{
-    if (n_gates < 0 || (n_gates && (!targets || !cmasks || !kinds)) || !n_sweeps || !n_passes) {
-        return einval("plan_dry_run: bad arguments");
-    }
-    return fused_plan_dry_run(n_qubits, precision, n_gates, targets, cmasks, kinds, n_sweeps, n_passes);
-}
-
 int b200sv_plan_gates(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2, const uint64_t* pmasks,
     const double* mats8, int* n_sweeps, int* n_passes, int* n_ops)
 {

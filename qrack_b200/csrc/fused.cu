@@ -26,6 +26,14 @@
 
 namespace b200sv {
 
+// the one kernel shape (DESIGN.md §7): a tile of 2^12 16-byte chunks, 256 threads, 2^4 register chunks per thread, 2 CTAs
+// per SM
+constexpr int FUSED_KC = 12;
+constexpr int FUSED_NT = 256;
+constexpr int FUSED_RB = 4;
+constexpr int FUSED_MINB = 2;
+constexpr int FUSED_L = 6; // low (contiguous) amplitude bits of a tile, both precisions
+
 constexpr int MAX_HIGH = 8;
 constexpr int MAX_PASS = 8;
 constexpr int MAX_OPS = 96;
@@ -92,7 +100,7 @@ struct alignas(16) DevSweep {
     double scale;
     int nOuter;   // outer-only phases (DevOuterPhase records at outerOff)
     int outerOff;
-    int prefetch; // 1: pull the CTA's next tile into L2 while this one is being computed
+    int reserved; // unused: kept because sizeof(DevSweep) counts against the program-size limit (how many ops fit a sweep)
     // scale: deferred scalar of the un-normalised Hadamard butterflies, applied once in the last pass
     int nSlots;   // per-tile phase table entries: slot 0 = tile scalar, slots 1.. = register-bit phases of the DIAG ops
     int scratchBytes; // shared memory behind the program: chunk-row offsets + the double-buffered phase table
@@ -184,11 +192,6 @@ template <> struct AmpOps<float> {
         x = f2add(x, y);
         y = f2fma(y, pk(-2.0f, -2.0f), x);
     }
-    static __device__ __forceinline__ void hadneg(A& x, A& y) // butterfly after a -1 phase on y: (x - y, x + y)
-    {
-        x = f2fma(y, pk(-1.0f, -1.0f), x);
-        y = f2fma(y, pk(2.0f, 2.0f), x);
-    }
     static __device__ __forceinline__ void rot(A& x, A& y, float c, float s)
     {
         const ull cc = pk(c, c), ss = pk(s, s), ns = pk(-s, -s);
@@ -237,13 +240,6 @@ template <> struct AmpOps<double> {
         y.x = fma(y.x, -2.0, x.x);
         y.y = fma(y.y, -2.0, x.y);
     }
-    static __device__ __forceinline__ void hadneg(A& x, A& y)
-    {
-        x.x -= y.x;
-        x.y -= y.y;
-        y.x = fma(y.x, 2.0, x.x);
-        y.y = fma(y.y, 2.0, x.y);
-    }
     static __device__ __forceinline__ void rot(A& x, A& y, double c, double s)
     {
         const A nx = make_double2(fma(c, x.x, -s * y.x), fma(c, x.y, -s * y.y));
@@ -279,15 +275,6 @@ template <typename R, int JR, int NA> __device__ __forceinline__ void app_rot(ty
     for (int e = 0; e < NA; ++e) {
         if (!(e & (1 << JR))) {
             O::rot(a[e], a[e | (1 << JR)], c, s);
-        }
-    }
-}
-template <typename R, int JR, int NA> __device__ __forceinline__ void app_hadneg(typename AmpOps<R>::A (&a)[NA])
-{
-#pragma unroll
-    for (int e = 0; e < NA; ++e) {
-        if (!(e & (1 << JR))) {
-            AmpOps<R>::hadneg(a[e], a[e | (1 << JR)]);
         }
     }
 }
@@ -356,13 +343,6 @@ template <typename R> struct alignas(16) DevMember {
     R ph[2];
 };
 
-// SV_NEG: fold a phase of exactly -1 that precedes a Hadamard on the same bit into a negative butterfly.  Off: the test adds
-// instructions to every stage and only saves phase applications that are rare in practice.
-#ifdef SV_NEG
-#define SV_NEG_OK true
-#else
-#define SV_NEG_OK false
-#endif
 template <typename R, int NA, int VAR>
 __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const DevOp<R>& op, const uint4 hd, uint32_t xsb,
     const R* __restrict__ tileScale, const DevMember<R>* __restrict__ members, const uint2* __restrict__ eff, const R* __restrict__ rotTab)
@@ -375,13 +355,13 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
 #define SV_J(J) (((1 << (J)) < NA) ? (J) : 0)
 #define SV_CASES(J)                                                                                                    \
     case K_XSWAP * 5 + J:                                                                                              \
-        app_xswap<R, SV_J(J), NA>(a, (uint32_t)em);                                                                           \
+        app_xswap<R, SV_J(J), NA>(a, em);                                                                              \
         break;                                                                                                         \
     case K_GEN_U * 5 + J:                                                                                              \
-        app_general<R, SV_J(J), NA, false>(a, m, (uint32_t)em);                                                                \
+        app_general<R, SV_J(J), NA, false>(a, m, em);                                                                  \
         break;                                                                                                         \
     case K_GEN_P * 5 + J:                                                                                              \
-        app_general<R, SV_J(J), NA, true>(a, m, (uint32_t)em);                                                                \
+        app_general<R, SV_J(J), NA, true>(a, m, em);                                                                   \
         break;
 #define SV_PAIR(K, J)                                                                                                  \
     case OPC_PH2 + (K) * ((K)-1) / 2 + (J):                                                                            \
@@ -393,18 +373,14 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
         const uint32_t hm = hd.y & ST_MASK, sm = (hd.y >> ST_SM_SHIFT) & ST_MASK, act = (hd.y >> ST_ACT_SHIFT) & ST_MASK,
                        rm = ROT ? ((hd.y >> ST_RM_SHIFT) & ST_MASK) : 0U;
         uint32_t slot = hd.z, mk = hd.w & 0xffffU, ri = hd.w >> 16;
-#ifndef SV_NO_FASTPATH
         if (!FULL && !(hd.y & (1U << ST_ANY_BIT))) {
             // the common shape: per-tile slot phases and butterflies only (no thread-level members)
 #define SV_STAGE_FAST(J)                                                                                               \
     if (((1 << (J)) < NA) && ((act >> (J)) & 1U)) {                                                                    \
-        bool neg = false;                                                                                              \
         if ((sm >> (J)) & 1U) {                                                                                        \
             const R px = tileScale[2U * slot], py = tileScale[2U * slot + 1U];                                         \
             ++slot;                                                                                                    \
-            /* a phase of exactly -1 right before a Hadamard on the same bit costs nothing: negative butterfly */      \
-            neg = SV_NEG_OK && (py == (R)0) && (px == (R)-1) && ((hm & ~rm) >> (J) & 1U);                              \
-            if (!neg && (px != (R)1 || py != (R)0)) {                                                                  \
+            if (px != (R)1 || py != (R)0) {                                                                            \
                 app_phase_reg<R, SV_J(J), NA>(a, O::mkph(px, py));                                                     \
             }                                                                                                          \
         }                                                                                                              \
@@ -412,8 +388,6 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
             if (ROT && ((rm >> (J)) & 1U)) {                                                                           \
                 app_rot<R, SV_J(J), NA>(a, rotTab[2U * ri], rotTab[2U * ri + 1U]);                                     \
                 ++ri;                                                                                                  \
-            } else if (neg) {                                                                                          \
-                app_hadneg<R, SV_J(J), NA>(a);                                                                         \
             } else {                                                                                                   \
                 app_had<R, SV_J(J), NA>(a);                                                                            \
             }                                                                                                          \
@@ -428,7 +402,6 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
 #undef SV_STAGE_FAST
             return;
         }
-#endif
         const uint32_t cnts = (hd.y & (1U << ST_ANY_BIT)) ? *reinterpret_cast<const uint32_t*>(op.m) : 0U;
         // product of the thread-level members [mk, mk + c) that fire for this thread, times (px, py)
 #define SV_MEMBERS(c)                                                                                                  \
@@ -458,7 +431,6 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
 #define SV_STAGE_BIT(J)                                                                                                \
     if (((1 << (J)) < NA) && ((act >> (J)) & 1U)) {                                                                    \
         const uint32_t c = (cnts >> (ST_CNT_BITS * ((J) + 1))) & ST_CNT_MASK;                                          \
-        bool neg = false;                                                                                              \
         if (((sm >> (J)) & 1U) | c) {                                                                                  \
             R px = (R)1, py = (R)0;                                                                                    \
             if ((sm >> (J)) & 1U) {                                                                                    \
@@ -467,8 +439,7 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
                 ++slot;                                                                                                \
             }                                                                                                          \
             SV_MEMBERS(c)                                                                                              \
-            neg = SV_NEG_OK && (py == (R)0) && (px == (R)-1) && ((hm & ~rm) >> (J) & 1U);                              \
-            if (!neg && (px != (R)1 || py != (R)0)) {                                                                  \
+            if (px != (R)1 || py != (R)0) {                                                                            \
                 app_phase_reg<R, SV_J(J), NA>(a, O::mkph(px, py));                                                     \
             }                                                                                                          \
         }                                                                                                              \
@@ -476,8 +447,6 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
             if (ROT && ((rm >> (J)) & 1U)) {                                                                           \
                 app_rot<R, SV_J(J), NA>(a, rotTab[2U * ri], rotTab[2U * ri + 1U]);                                     \
                 ++ri;                                                                                                  \
-            } else if (neg) {                                                                                          \
-                app_hadneg<R, SV_J(J), NA>(a);                                                                         \
             } else {                                                                                                   \
                 app_had<R, SV_J(J), NA>(a);                                                                            \
             }                                                                                                          \
@@ -497,8 +466,8 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
     if (hd.x & CODE_HAS_SB) {
         tp = (xsb & hd.z) == hd.w;
     }
-    // register-amplitude predicate mask (64 bits when the sub-block holds 64 amplitudes: high word = third word of op.m)
-    const uint64_t em = tp ? ((uint64_t)hd.y | ((NA > 32) ? ((uint64_t)reinterpret_cast<const uint32_t*>(op.m)[2] << 32) : 0ULL)) : 0ULL;
+    // register-amplitude predicate mask
+    const uint32_t em = tp ? hd.y : 0U;
     if (FULL && (hd.x & 0xffU) < OPC_PHGEN) {
         switch (hd.x & 0xffU) {
             SV_CASES(0)
@@ -539,7 +508,7 @@ __device__ __forceinline__ void exec_op(typename AmpOps<R>::A (&a)[NA], const De
 #pragma unroll
         for (int e = 0; e < NA; ++e) {
             const A v = O::mulc(a[e], ph);
-            a[e] = ((em >> e) & 1ULL) ? v : a[e];
+            a[e] = ((em >> e) & 1U) ? v : a[e];
         }
     } break;
     default:
@@ -576,12 +545,13 @@ template <typename C> __device__ __forceinline__ const C* pull_src(const PullArg
     return reinterpret_cast<const C*>(pa.peers[r]) + ((i & ~pa.vmask) | pa.rankDep);
 }
 
-template <typename R, int NT>
+template <typename R>
 __device__ __noinline__ void stage_in_pull(const PullArgs& pa, uint64_t base, unsigned char* tileB, const uint64_t* rowOff,
     uint32_t nChunk, int lcb, uint32_t colMask, int tid)
 {
     typedef typename Cx<R>::type C;
     constexpr int APC = AmpOps<R>::APC;
+    constexpr int NT = FUSED_NT;
     for (uint32_t c0 = (uint32_t)tid; c0 < nChunk; c0 += 4U * NT) {
         uint4 v[4];
 #pragma unroll
@@ -601,11 +571,12 @@ __device__ __noinline__ void stage_in_pull(const PullArgs& pa, uint64_t base, un
     }
 }
 
-template <typename R, int NT>
+template <typename R>
 __device__ __noinline__ void stage_in(const typename Cx<R>::type* __restrict__ tilePsi, unsigned char* tileB, const uint64_t* rowOff,
     uint32_t nChunk, int lcb, uint32_t colMask, int tid)
 {
     constexpr int APC = AmpOps<R>::APC;
+    constexpr int NT = FUSED_NT;
     if (nChunk >= 8U * NT) {
         for (uint32_t c0 = (uint32_t)tid; c0 < nChunk; c0 += 8U * NT) {
             uint4 v[8];
@@ -627,11 +598,12 @@ __device__ __noinline__ void stage_in(const typename Cx<R>::type* __restrict__ t
         }
     }
 }
-template <typename R, int NT>
+template <typename R>
 __device__ __noinline__ void stage_out(typename Cx<R>::type* __restrict__ tilePsi, const unsigned char* tileB, const uint64_t* rowOff,
     uint32_t nChunk, int lcb, uint32_t colMask, int tid)
 {
     constexpr int APC = AmpOps<R>::APC;
+    constexpr int NT = FUSED_NT;
 #pragma unroll 4
     for (uint32_t c = (uint32_t)tid; c < nChunk; c += NT) {
         st_stream(reinterpret_cast<uint4*>(tilePsi + rowOff[c >> lcb] + (uint64_t)(c & colMask) * APC),
@@ -641,8 +613,8 @@ __device__ __noinline__ void stage_out(typename Cx<R>::type* __restrict__ tilePs
 
 // PULL: the sweep also performs a pending re-page (PullArgs): its first pass (or the staged tile copy) reads every chunk through
 // the peer mapping that holds it, its last pass writes this rank's other page; everything between is unchanged.
-template <typename R, int KC, int RB, int NT, int MINB, int VAR, bool PULL = false>
-__global__ void __launch_bounds__(NT, MINB)
+template <typename R, int VAR, bool PULL = false>
+__global__ void __launch_bounds__(FUSED_NT, FUSED_MINB)
     k_fused_sweep(typename Cx<R>::type* __restrict__ psi, const unsigned char* __restrict__ prog, uint32_t progBytes, uint64_t nTiles,
         const __grid_constant__ PullArgs pull)
 {
@@ -651,13 +623,14 @@ __global__ void __launch_bounds__(NT, MINB)
     typedef typename O::A A;
     typedef typename O::Chunk Chunk;
     constexpr int APC = O::APC;
-    constexpr int NCH = 1 << RB;
+    constexpr int NT = FUSED_NT;
+    constexpr int NCH = 1 << FUSED_RB;
     constexpr int NA = NCH * APC;
     static_assert(NA <= MAX_NA && NCH <= MAX_NCH, "register sub-block too large");
-    static_assert(NT >= 128, "the per-tile preamble uses warps 0..3 for the ballots and the tile scalar");
+    static_assert(NT > 128, "the per-tile preamble uses warps 0..3 for the ballots and the tile scalar, the rest for the table slots");
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char* tileB = smem;
-    unsigned char* sprog = smem + ((size_t)16 << KC);
+    unsigned char* sprog = smem + ((size_t)16 << FUSED_KC);
     __shared__ uint32_t ballots[2][4]; // double-buffered by tile parity (like tileTab) so that one barrier per tile is enough
 
     const int tid = threadIdx.x;
@@ -686,7 +659,7 @@ __global__ void __launch_bounds__(NT, MINB)
         }
         rowOff[r] = off;
     }
-    const uint32_t nSub = nChunk >> RB;
+    const uint32_t nSub = nChunk >> FUSED_RB;
     const int nOps = sw.nOps;
     const int nOuter = sw.nOuter;
     const int nPass = sw.nPass;
@@ -710,8 +683,14 @@ __global__ void __launch_bounds__(NT, MINB)
     }
     __syncthreads();
 
-    uint32_t par = 0;
-    for (uint64_t t = blockIdx.x; t < nTiles; t += gridDim.x, par ^= 1U) {
+    // tile t = blockIdx.x + k * gridDim.x; only the 32-bit k is carried across tiles (a CTA never sees 2^32 64 KB tiles of a state
+    // that fits in device memory), which keeps one more register free for the pass loop
+    for (uint32_t k = 0;; ++k) {
+        const uint64_t t = blockIdx.x + (uint64_t)k * gridDim.x;
+        if (t >= nTiles) {
+            break;
+        }
+        const uint32_t par = k & 1U;
         uint64_t base = t << sw.lowAmpBits;
         for (int h = 0; h < sw.nHigh; ++h) {
             const uint64_t lo = base & sw.highLow[h];
@@ -753,8 +732,8 @@ __global__ void __launch_bounds__(NT, MINB)
             }
         }
         // table slots 1..: product (in double) of the member phases that fire for this tile; one thread per slot, the threads
-        // beyond the four role warps first (NT = 256), everybody when the CTA has only those four (NT = 128)
-        for (int sl = 1 + ((NT > 128) ? (tid >= 128 ? tid - 128 : tid + NT - 128) : tid); sl < sw.nSlots; sl += NT) {
+        // beyond the four role warps first
+        for (int sl = 1 + (tid >= 128 ? tid - 128 : tid + NT - 128); sl < sw.nSlots; sl += NT) {
             double fx = 1.0, fy = 0.0;
             for (int i = sw.slotBeg[sl], e = sw.slotBeg[sl + 1]; i < e; ++i) {
                 const DevOuterPhase<R>& op = outer[i];
@@ -776,26 +755,15 @@ __global__ void __launch_bounds__(NT, MINB)
                 eff[i] = ok ? make_uint2(mb.lmask, mb.lval) : make_uint2(0U, 1U);
             }
         }
-        if (!PULL && sw.prefetch && (t + gridDim.x < nTiles) && ((tid & 7) == 0)) {
-            // one 128-byte line per 8 chunks: the CTA's next tile streams into L2 under the passes below
-            uint64_t nb = (t + gridDim.x) << sw.lowAmpBits;
-            for (int h = 0; h < sw.nHigh; ++h) {
-                const uint64_t lo = nb & sw.highLow[h];
-                nb = ((nb ^ lo) << 1) | lo;
-            }
-            for (uint32_t c = (uint32_t)tid; c < nChunk; c += NT) {
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(psi + nb + rowOff[c >> lcb] + (uint64_t)(c & colMask) * APC));
-            }
-        }
         if (!sw.directIn) {
             // staged input (register bits of the first pass sit on low chunk bits, where per-thread HBM access would
             // split sectors): coalesced copy global -> swizzled smem.  The extra barrier keeps slow warps of the
             // previous tile from still reading the tile area.
             __syncthreads();
             if (PULL) {
-                stage_in_pull<R, NT>(pull, base, tileB, rowOff, nChunk, lcb, colMask, tid);
+                stage_in_pull<R>(pull, base, tileB, rowOff, nChunk, lcb, colMask, tid);
             } else {
-                stage_in<R, NT>(tilePsi, tileB, rowOff, nChunk, lcb, colMask, tid);
+                stage_in<R>(tilePsi, tileB, rowOff, nChunk, lcb, colMask, tid);
             }
         }
         // The barrier publishes the tables (and the staged tile) and closes the previous tile: nobody still reads the
@@ -866,7 +834,7 @@ __global__ void __launch_bounds__(NT, MINB)
         }
         if (!sw.directOut) {
             // staged output: swizzled smem -> global, coalesced (the barrier above closed the last pass)
-            stage_out<R, NT>(tilePsi, tileB, rowOff, nChunk, lcb, colMask, tid);
+            stage_out<R>(tilePsi, tileB, rowOff, nChunk, lcb, colMask, tid);
         }
     }
 }
@@ -886,11 +854,9 @@ struct HostOp {
 static inline uint64_t bitq(int q) { return 1ULL << q; }
 
 static uint64_t rewrite_ops(std::vector<HostOp>& ops);
-static int knob_rewrite();
 // returns the mask of a trailing XMask that is better served by the dedicated sweep (launch_xmask) after the fused sweeps
 static uint64_t lower_queue(const std::vector<GateOp>& q, std::vector<HostOp>& out)
 {
-    uint64_t xtail = 0;
     out.clear();
     out.reserve(q.size() * 2);
     for (const GateOp& g : q) {
@@ -899,7 +865,7 @@ static uint64_t lower_queue(const std::vector<GateOp>& q, std::vector<HostOp>& o
         if (g.kind == 1) { // diagonal: one predicated phase per non-unit diagonal entry
             const bool one0 = (g.m[0] == 1.0 && g.m[1] == 0.0), one3 = (g.m[6] == 1.0 && g.m[7] == 0.0);
             const double n0 = g.m[0] * g.m[0] + g.m[1] * g.m[1];
-            if (knob_rewrite() && !one0 && n0 > 0.0) {
+            if (!one0 && n0 > 0.0) {
                 // diag(d0, d3) under controls C  =  [C -> d0] . [C and target=1 -> d3 / d0]: every register-bit predicate the
                 // kernel sees then asks for value 1 (a stage member), and the first factor has one qubit less
                 h.kind = OP_PHASE;
@@ -919,6 +885,7 @@ static uint64_t lower_queue(const std::vector<GateOp>& q, std::vector<HostOp>& o
                 }
                 continue;
             }
+            // d0 = 1 (or |d0| = 0): one predicated phase per remaining non-unit entry
             if (!one0) {
                 h.kind = OP_PHASE;
                 h.tq = -1;
@@ -953,9 +920,7 @@ static uint64_t lower_queue(const std::vector<GateOp>& q, std::vector<HostOp>& o
         }
         out.push_back(h);
     }
-    if (knob_rewrite()) {
-        xtail = rewrite_ops(out);
-    }
+    const uint64_t xtail = rewrite_ops(out);
     if (getenv("B200SV_FUSED_DEBUG")) {
         int cnt[5] = { 0, 0, 0, 0, 0 };
         for (const HostOp& h : out) {
@@ -1013,8 +978,6 @@ static inline bool is_had_form(const double* m)
 {
     return m[1] == 0.0 && m[3] == 0.0 && m[5] == 0.0 && m[7] == 0.0 && m[0] > 0.0 && m[0] == m[2] && m[0] == m[4] && m[6] == -m[0];
 }
-static int knob_rewrite();
-static int knob_rot();
 
 static uint64_t rewrite_ops(std::vector<HostOp>& ops)
 {
@@ -1221,13 +1184,12 @@ static uint64_t rewrite_ops(std::vector<HostOp>& ops)
     // and are applied lazily.  Quantum-volume layers (AI gates + CNOTs) become rotations + phases only: the flush is "light".
     std::vector<HostOp> res;
     res.reserve(out.size() + 1);
-    const bool rot = knob_rot() != 0;
     for (size_t i = 0; i < out.size(); ++i) {
         if (!alive[i]) {
             continue;
         }
         const HostOp& h = out[i];
-        if (rot && h.kind == OP_GENERAL && !h.cmask) {
+        if (h.kind == OP_GENERAL && !h.cmask) {
             const double* m = h.m;
             const double n00 = m[0] * m[0] + m[1] * m[1], n10 = m[4] * m[4] + m[5] * m[5];
             const double n01 = m[2] * m[2] + m[3] * m[3], n11 = m[6] * m[6] + m[7] * m[7];
@@ -1293,35 +1255,27 @@ static uint64_t rewrite_ops(std::vector<HostOp>& ops)
 struct TileCfg {
     int n;    // qubits
     int apcLog; // 1 for fp32, 0 for fp64
-    int KC;   // max tile chunk bits
-    int RB;   // register chunk bits per pass
     int L;    // low (contiguous) amplitude bits
     int kA;   // tile amplitude bits actually used
     int H;    // capacity of high qubits
-    int NT;   // threads per CTA
-    int maxOps; // ops per sweep (bounded by the shared-memory program area: 3 CTAs/SM must fit)
-    int bundle; // bit 0: merge Hadamards on distinct register bits into one LAYER op
+    int maxOps; // ops per sweep (bounded by the shared-memory program area)
     // virtual qubits (>= n, State::nVirt): constant on this state; predicates on them are folded when the sweep is encoded
     uint64_t virtMask = 0, virtVal = 0;
 };
 
-static TileCfg make_cfg(int n, int prec, int KC, int RB, int Lpref, int NT = 256)
+static TileCfg make_cfg(int n, int prec)
 {
     TileCfg c;
-    c.NT = NT;
     c.n = n;
     c.apcLog = (prec == 32) ? 1 : 0;
-    c.KC = KC;
-    c.RB = RB;
-    const int kAmax = KC + c.apcLog;
+    const int kAmax = FUSED_KC + c.apcLog;
     c.kA = std::min(n, kAmax);
-    c.L = std::min(Lpref, c.kA);
+    c.L = std::min(FUSED_L, c.kA);
     if (n <= kAmax) {
         c.L = c.kA; // whole state is one tile
     }
     c.H = c.kA - c.L;
     c.maxOps = MAX_HOST_OPS;
-    c.bundle = 7;
     return c;
 }
 
@@ -1329,13 +1283,13 @@ static TileCfg make_cfg(int n, int prec, int KC, int RB, int Lpref, int NT = 256
 //   fits(op)   : can the op be executed under the current resource set (may grow the set)
 // Ops that are skipped block later ops that do not commute with them.
 // Lazy diagonals (r2): a diagonal op commutes with everything except a non-diagonal op on one of its qubits, so it may be
-// applied anywhere between its neighbours of that kind.  With `lazy`, a diagonal op is taken at once only when it costs
+// applied anywhere between its neighbours of that kind.  So a diagonal op is taken at once only when it costs
 // nothing here (isFree: none of its qubits is a tile qubit -> per-tile scalar); otherwise it is DEFERRED without blocking
 // anything, and pulled in right before the first taken non-diagonal op that acts on one of its qubits (so its phase joins
 // the stage of that butterfly instead of costing a phase application of its own), or left for a later pass / sweep where it
 // may be free.  When no non-diagonal op remains, the deferred ones are taken (progress, and no diagonal-only extra sweep).
 template <typename FitFn, typename FreeFn>
-static void greedy_select(std::vector<HostOp>& pending, std::vector<HostOp>& taken, size_t maxTake, size_t lookahead, FitFn fits, bool lazy,
+static void greedy_select(std::vector<HostOp>& pending, std::vector<HostOp>& taken, size_t maxTake, size_t lookahead, FitFn fits,
     FreeFn isFree)
 {
     uint64_t blockedT = 0, blockedD = 0;
@@ -1352,7 +1306,7 @@ static void greedy_select(std::vector<HostOp>& pending, std::vector<HostOp>& tak
         const uint64_t usesT = op.tq >= 0 ? bitq(op.tq) : 0;
         const uint64_t usesD = op.cmask;
         bool conflict = (usesT & (blockedT | blockedD)) || (usesD & blockedT);
-        if (!conflict && lazy && op.kind == OP_PHASE && !isFree(op)) {
+        if (!conflict && op.kind == OP_PHASE && !isFree(op)) {
             deferred.push_back(i);
             deferredQ |= usesD;
             continue;
@@ -1394,7 +1348,7 @@ static void greedy_select(std::vector<HostOp>& pending, std::vector<HostOp>& tak
     for (size_t k = i; k < pending.size() && !nonDiagLeft; ++k) {
         nonDiagLeft = pending[k].kind != OP_PHASE;
     }
-    if (lazy && !nonDiagLeft) {
+    if (!nonDiagLeft) {
         // only diagonal ops are left: take them now, in order
         for (size_t k = 0; k < pending.size() && taken.size() < maxTake; ++k) {
             if (!gone[k]) {
@@ -1426,7 +1380,6 @@ struct SweepPlan {
 
 // Count-only twin of greedy_select for a FIXED tile (no copies): how many of the first `lookahead` pending ops could run in
 // a sweep whose tile qubits are `inTile`.
-static int knob_plan_weight();
 static size_t greedy_count(const std::vector<HostOp>& pending, size_t maxTake, size_t lookahead, uint64_t inTile)
 {
     uint64_t blockedT = 0, blockedD = 0;
@@ -1443,15 +1396,15 @@ static size_t greedy_count(const std::vector<HostOp>& pending, size_t maxTake, s
                 break; // every tile qubit is blocked: only stray diagonal gates could still be taken
             }
         } else {
-            // objective of the search: non-diagonal ops weigh `w`, diagonal ops 1 (knob B200SV_PLAN_WEIGHT, default 1 = plain count)
-            taken += (op.kind == OP_PHASE) ? 1U : (size_t)knob_plan_weight();
+            ++taken;
         }
     }
     return taken;
 }
 
-static int knob_plan_search();
-static int knob_lazy_diag();
+// hill-climbing rounds of the tile-qubit and register-qubit search.  On BASELINE's 30-qubit random circuit the search packs
+// the 1800 gates into 38 sweeps instead of 51 (138 passes instead of 156) for ~3 ms of planning.
+constexpr int SEARCH_ROUNDS = 2;
 
 static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPlan& sp)
 {
@@ -1459,10 +1412,7 @@ static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPl
     uint64_t inTile = (cfg.L >= 64) ? ~0ULL : (bitq(cfg.L) - 1U);
     int freeHigh = cfg.H;
     std::vector<HostOp> sel;
-    // B200SV_PLAN_SEARCH = hill-climbing rounds (default 2, 0 = first-use order only).  On BASELINE's 30-qubit random circuit
-    // the search packs the 1800 gates into 38 sweeps instead of 51 (138 passes instead of 156) for ~3 ms of planning.
-    const int searchRounds = knob_plan_search();
-    if (searchRounds > 0 && cfg.H > 0 && cfg.n > cfg.L + cfg.H) {
+    if (cfg.H > 0 && cfg.n > cfg.L + cfg.H) {
         // hill-climb on the set of high qubits: start from the order-of-first-use choice, swap one member at a time
         const uint64_t lowMask = inTile;
         uint64_t cur = lowMask;
@@ -1488,7 +1438,7 @@ static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPl
             }
         }
         size_t best = greedy_count(pending, (size_t)cfg.maxOps, 2048, cur);
-        for (int round = 0; round < searchRounds; ++round) {
+        for (int round = 0; round < SEARCH_ROUNDS; ++round) {
             uint64_t bestSet = cur;
             for (int h = cfg.L; h < cfg.n; ++h) {
                 if (!(cur & bitq(h))) {
@@ -1514,7 +1464,6 @@ static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPl
         inTile = cur;
         freeHigh = 0;
     }
-    const bool lazy = knob_lazy_diag() != 0;
     greedy_select(
         pending, sel, (size_t)cfg.maxOps, 2048,
         [&](const HostOp& op) {
@@ -1528,7 +1477,7 @@ static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPl
             }
             return false;
         },
-        lazy, [&](const HostOp& op) { return freeHigh == 0 && !(op.cmask & inTile); });
+        [&](const HostOp& op) { return freeHigh == 0 && !(op.cmask & inTile); });
     sp.highQ.clear();
     for (int q = cfg.L; q < cfg.n; ++q) {
         if (inTile & bitq(q)) {
@@ -1549,52 +1498,48 @@ static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPl
     while (!sel.empty() && (int)sp.passes.size() < MAX_PASS) {
         PassPlan pp;
         uint64_t regSet = cfg.apcLog ? 1ULL : 0ULL; // fp32: qubit 0 is always register-resident
-        int freeReg = cfg.RB;
-        if (searchRounds > 0) {
-            // same hill climbing for the pass's register qubits (targets must be register-resident, everything else rides along)
-            const uint64_t fixed = regSet;
-            uint64_t cur = fixed;
-            {
-                int fr = cfg.RB;
-                uint64_t bT = 0, bD = 0;
-                for (size_t i = 0; i < sel.size() && fr > 0; ++i) {
-                    const HostOp& op = sel[i];
-                    const uint64_t uT = op.tq >= 0 ? bitq(op.tq) : 0, uD = op.cmask;
-                    if ((uT & (bT | bD)) || (uD & bT)) {
-                        bT |= uT;
-                        bD |= uD;
-                    } else if (uT & ~cur) {
-                        cur |= uT;
-                        --fr;
+        int freeReg = FUSED_RB;
+        // same hill climbing for the pass's register qubits (targets must be register-resident, everything else rides along)
+        const uint64_t fixed = regSet;
+        uint64_t cur = fixed;
+        int fr = FUSED_RB;
+        uint64_t bT = 0, bD = 0;
+        for (size_t i = 0; i < sel.size() && fr > 0; ++i) {
+            const HostOp& op = sel[i];
+            const uint64_t uT = op.tq >= 0 ? bitq(op.tq) : 0, uD = op.cmask;
+            if ((uT & (bT | bD)) || (uD & bT)) {
+                bT |= uT;
+                bD |= uD;
+            } else if (uT & ~cur) {
+                cur |= uT;
+                --fr;
+            }
+        }
+        if (fr == 0) { // only worth searching when the pass is register-limited
+            size_t best = greedy_count(sel, (size_t)cfg.maxOps, 4096, cur);
+            for (int round = 0; round < SEARCH_ROUNDS; ++round) {
+                uint64_t bestSet = cur;
+                for (uint64_t hm = cur & ~fixed; hm; hm &= hm - 1U) {
+                    const uint64_t hbit = hm & (~hm + 1U);
+                    for (uint64_t cm = inTile & ~cur; cm; cm &= cm - 1U) {
+                        const uint64_t cbit = cm & (~cm + 1U);
+                        const uint64_t cand = (cur & ~hbit) | cbit;
+                        const size_t got = greedy_count(sel, (size_t)cfg.maxOps, 4096, cand);
+                        if (got > best) {
+                            best = got;
+                            bestSet = cand;
+                        }
                     }
                 }
-                if (fr == 0) { // only worth searching when the pass is register-limited
-                    size_t best = greedy_count(sel, (size_t)cfg.maxOps, 4096, cur);
-                    for (int round = 0; round < searchRounds; ++round) {
-                        uint64_t bestSet = cur;
-                        for (uint64_t hm = cur & ~fixed; hm; hm &= hm - 1U) {
-                            const uint64_t hbit = hm & (~hm + 1U);
-                            for (uint64_t cm = inTile & ~cur; cm; cm &= cm - 1U) {
-                                const uint64_t cbit = cm & (~cm + 1U);
-                                const uint64_t cand = (cur & ~hbit) | cbit;
-                                const size_t got = greedy_count(sel, (size_t)cfg.maxOps, 4096, cand);
-                                if (got > best) {
-                                    best = got;
-                                    bestSet = cand;
-                                }
-                            }
-                        }
-                        if (bestSet == cur) {
-                            break;
-                        }
-                        cur = bestSet;
-                    }
-                    regSet = cur;
-                    freeReg = 0;
-                    for (uint64_t m = cur & ~fixed; m; m &= m - 1U) {
-                        pp.regQ.push_back(__builtin_ctzll(m));
-                    }
+                if (bestSet == cur) {
+                    break;
                 }
+                cur = bestSet;
+            }
+            regSet = cur;
+            freeReg = 0;
+            for (uint64_t m = cur & ~fixed; m; m &= m - 1U) {
+                pp.regQ.push_back(__builtin_ctzll(m));
             }
         }
         greedy_select(
@@ -1611,7 +1556,7 @@ static void plan_sweep(std::vector<HostOp>& pending, const TileCfg& cfg, SweepPl
                 }
                 return false;
             },
-            lazy, [&](const HostOp& op) { return !(op.cmask & inTile); });
+            [&](const HostOp& op) { return !(op.cmask & inTile); });
         sp.passes.push_back(pp);
     }
     if (!sel.empty()) {
@@ -1636,20 +1581,16 @@ static int tile_bit(const TileCfg& cfg, const std::vector<int>& highQ, int q)
     return -1;
 }
 
-// Encoded size limits of one sweep program (must fit beside the tile in shared memory with 3 CTAs/SM)
-constexpr size_t MAX_PROG_BYTES_3CTA = 10240; // (227 KB / 3) - 64 KB tile - 1 KB reserved - static
+// Encoded size limit of one sweep program plus its scratch (fits beside the 64 KB tile in shared memory with 2 CTAs/SM)
 constexpr size_t MAX_PROG_BYTES_2CTA = 24576;
 
-static int knob_prefetch();
-static int knob_direct_low();
 template <typename R>
 static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<unsigned char>& buf, size_t* scratchOut)
 {
     const int kc = cfg.kA - cfg.apcLog;
     const int APC = 1 << cfg.apcLog;
-    const int NCH = 1 << cfg.RB;
+    const int NCH = 1 << FUSED_RB;
     const int NA = NCH * APC;
-    const int NT = cfg.NT;
     int JRN = 0;
     while ((1 << JRN) < NA) {
         ++JRN;
@@ -1683,7 +1624,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
             rb.push_back(cb);
             used |= 1U << cb;
         }
-        for (int cb = kc - 1; cb >= 0 && (int)rb.size() < cfg.RB; --cb) {
+        for (int cb = kc - 1; cb >= 0 && (int)rb.size() < FUSED_RB; --cb) {
             if (!(used & (1U << cb))) {
                 rb.push_back(cb);
                 used |= 1U << cb;
@@ -1713,9 +1654,9 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
             dp.sbit[i] = (unsigned char)sb[i];
         }
         const uint32_t nSub = 1U << dp.nsb;
-        dp.nIt = (int)std::max<uint32_t>(1U, nSub / (uint32_t)NT);
+        dp.nIt = (int)std::max<uint32_t>(1U, nSub / (uint32_t)FUSED_NT);
         int tidBits = 0;
-        while ((1 << tidBits) < NT) {
+        while ((1 << tidBits) < FUSED_NT) {
             ++tidBits;
         }
         for (int it = 0; it < dp.nIt && it < 16; ++it) {
@@ -1735,7 +1676,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
         }
         for (int e = 0; e < NCH; ++e) {
             uint32_t off = 0;
-            for (int b = 0; b < cfg.RB; ++b) {
+            for (int b = 0; b < FUSED_RB; ++b) {
                 if ((e >> b) & 1) {
                     off |= 1U << rb[b];
                 }
@@ -1754,7 +1695,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
                 roffA[e * APC + w] = (off << cfg.apcLog) | (uint32_t)w;
             }
         }
-        const uint64_t fullE = (NA >= 64) ? ~0ULL : ((1ULL << NA) - 1ULL);
+        const uint32_t fullE = (uint32_t)((1ULL << NA) - 1ULL);
         auto reg_index = [&](int tb) {
             int jr = 0;
             for (int b = 0; b < tb; ++b) {
@@ -1881,7 +1822,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
                     outerList.push_back(op);
                     continue;
                 }
-                if ((cfg.bundle & 2) && nreg <= 1 && lvr == lmr) {
+                if (nreg <= 1 && lvr == lmr) {
                     // stage member: at most one register bit (value 1); thread bits and outer qubits anywhere
                     const int jr = nreg ? reg_index(__builtin_ctz(lmr)) : -1;
                     const bool threadPart = (lmask & ~regAmpMask) != 0;
@@ -1917,14 +1858,11 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
                             st.thr[jr + 1].push_back(mem);
                         }
                         st.any = true;
-                        if (!(cfg.bundle & 4)) {
-                            close_stage();
-                        }
                         continue;
                     }
                     // tables full: falls through to a single op
                 }
-            } else if ((cfg.bundle & 1) && !hop.cmask && (hop.kind == OP_HAD || hop.kind == OP_ROT)) {
+            } else if (!hop.cmask && (hop.kind == OP_HAD || hop.kind == OP_ROT)) {
                 // uncontrolled Hadamard / real rotation: butterfly of the stage (after the stage's phase on that bit)
                 const int jr = reg_index(tile_bit(cfg, sp.highQ, hop.tq));
                 if (st.h[jr] || rotList.size() / 2U + 8U >= 65535U) {
@@ -1939,15 +1877,12 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
                 } else {
                     scale *= hop.m[0];
                 }
-                if (!(cfg.bundle & 4)) {
-                    close_stage();
-                }
                 continue;
             }
             // everything else is a single op, emitted at once: the open stage has to be closed first if the op does not
             // commute with its contents (target bit: any member; register-bit controls / phased register bits: a butterfly)
             {
-                bool conflict = !(cfg.bundle & 4);
+                bool conflict = false;
                 if (hop.tq >= 0) {
                     const int jt = reg_index(tile_bit(cfg, sp.highQ, hop.tq));
                     conflict = conflict || st.h[jt] || !st.slot[jt].empty() || !st.thr[jt + 1].empty();
@@ -1965,20 +1900,16 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
             d.oval = hop.cval & ~tileMask;
             d.lmaskSb = lmask & ~regAmpMask;
             d.lvalSb = lval & ~regAmpMask;
-            uint64_t em = 0;
+            uint32_t em = 0;
             for (int e = 0; e < NA; ++e) {
                 if ((roffA[e] & lmr) == lvr) {
-                    em |= 1ULL << e;
+                    em |= 1U << e;
                 }
             }
-            d.emask = (uint32_t)em;
+            d.emask = em;
             const bool uncond = (em == fullE && d.lmaskSb == 0);
             for (int k = 0; k < 8; ++k) {
                 d.m[k] = (R)hop.m[k];
-            }
-            if (NA > 32) { // 64 register amplitudes (fp32, RB = 5; phase ops only): the high half of the mask rides in the third word of m
-                const uint32_t hi = (uint32_t)(em >> 32);
-                memcpy(reinterpret_cast<unsigned char*>(d.m) + 8, &hi, sizeof(hi));
             }
             uint32_t code = 0;
             if (hop.kind == OP_PHASE) {
@@ -1990,21 +1921,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
                 }
             } else {
                 const uint32_t jr = (uint32_t)reg_index(tile_bit(cfg, sp.highQ, hop.tq));
-                if (hop.kind == OP_HAD || hop.kind == OP_ROT) {
-                    // only with stage bundling switched off for butterflies: a stage of its own
-                    close_stage();
-                    st.h[jr] = true;
-                    st.any = true;
-                    if (hop.kind == OP_ROT) {
-                        st.isRot[jr] = true;
-                        st.rc[jr] = hop.m[0];
-                        st.rs[jr] = hop.m[1];
-                    } else {
-                        scale *= hop.m[0];
-                    }
-                    close_stage();
-                    continue;
-                } else if (hop.kind == OP_XSWAP) {
+                if (hop.kind == OP_XSWAP) {
                     code = K_XSWAP * 5U + jr;
                 } else {
                     code = (uncond ? K_GEN_U : K_GEN_P) * 5U + jr;
@@ -2036,9 +1953,9 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
             }
             return cnt;
         };
-        const int dlow = knob_direct_low();
-        ds.directIn = (lowRegBits(sp.passes.front()) <= dlow) ? 1 : 0;
-        ds.directOut = (lowRegBits(sp.passes.back()) <= dlow) ? 1 : 0;
+        // the first / last pass goes straight HBM <-> registers when at most one of its register bits is a chunk bit 0..2
+        ds.directIn = (lowRegBits(sp.passes.front()) <= 1) ? 1 : 0;
+        ds.directOut = (lowRegBits(sp.passes.back()) <= 1) ? 1 : 0;
     }
     ds.scale = scale;
     if (getenv("B200SV_FUSED_DEBUG")) {
@@ -2077,7 +1994,6 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
         fprintf(stderr, "  sweep: %d ops, %d outer phases, %d thread members, directIn %d, directOut %d\n", (int)dops.size(),
             (int)outerList.size(), (int)memberList.size(), ds.directIn, ds.directOut);
     }
-    ds.prefetch = knob_prefetch();
     ds.hasScale = (scale != 1.0 || !outerList.empty()) ? 1 : 0;
     ds.nOps = (int)dops.size();
     ds.nOuter = (int)outerList.size();
@@ -2088,7 +2004,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
         const size_t rows = (size_t)1 << (kc > lcb ? kc - lcb : 0);
         ds.scratchBytes =
             (int)((rows * 8U + (size_t)4 * (size_t)ds.nSlots * sizeof(R) + (size_t)16 * memberList.size() +
-                      (size_t)2 * (size_t)ds.nPass * (size_t)NT + 15U) & ~(size_t)15U); // + per-(pass, thread) sub-block bases
+                      (size_t)2 * (size_t)ds.nPass * (size_t)FUSED_NT + 15U) & ~(size_t)15U); // + per-(pass, thread) sub-block bases
     }
     ds.nMem = (int)memberList.size();
     ds.slotBeg[0] = 0;
@@ -2151,8 +2067,7 @@ static int plan_and_encode(std::vector<HostOp>& pending, const TileCfg& cfg0, in
         size_t scratch = 0;
         const size_t bytes =
             (prec == 32) ? encode_sweep<float>(sp, cfg, buf, &scratch) : encode_sweep<double>(sp, cfg, buf, &scratch);
-        const size_t limit = (cfg.RB >= 4) ? MAX_PROG_BYTES_2CTA : MAX_PROG_BYTES_3CTA;
-        if (bytes + scratch > limit) {
+        if (bytes + scratch > MAX_PROG_BYTES_2CTA) {
             if (cfg.maxOps <= 4) {
                 set_error("fused sweep program does not fit");
                 return B200SV_ESTATE;
@@ -2246,7 +2161,7 @@ static int plan_list(std::vector<HostOp>& pending, const TileCfg& cfg, int prec,
 // Plans and encodes every sweep of a flush.
 //
 // With `carry` the under-filled tail of the window is not executed.  Phase A decides WHAT is handed back, on the symbolic op list
-// (virtual-qubit predicates unfolded), so that every rank of a sharded register — same queue, same knobs, deterministic planner —
+// (virtual-qubit predicates unfolded), so that every rank of a sharded register — same queue, deterministic planner —
 // takes the same decision: an exchange redistributes amplitudes between the ranks, an op executed before it on one rank and after
 // it on another would hit some amplitudes twice.  Candidate cuts: j = first sweep of a trailing run of sweeps that each hold fewer
 // than minOps ops.  Of what is left over at cut j (program order) the ops that MUST still run now are the non-diagonal ops on
@@ -2355,7 +2270,7 @@ static int plan_all(std::vector<HostOp>& pending, const TileCfg& cfg, int prec, 
             exec[w++] = h;
         }
         exec.resize(w);
-        if (changed && knob_rewrite()) {
+        if (changed) {
             // the peephole rules once more on what is left: the Hadamard pair around a controlled-X whose rank-bit control fails here is
             // H . H now, a CZ that lost its rank-bit control is a Z to absorb, ...
             *xtail ^= rewrite_ops(exec);
@@ -2428,24 +2343,19 @@ void fused_release(State* s)
 
 bool fused_accepts(const State* s, const GateOp&) { return s->nq >= 5 && s->nq <= 62; }
 
-struct KernelCfg {
-    int KC, RB, NT, MINB;
-};
-
-template <typename R, int KC, int RB, int NT, int MINB, int VAR, bool PULL = false>
+template <typename R, int VAR, bool PULL = false>
 static int launch_sweep_v(State* s, const unsigned char* dprog, uint32_t progBytes, uint32_t scratchBytes, uint64_t nTiles)
 {
-    auto kern = k_fused_sweep<R, KC, RB, NT, MINB, VAR, PULL>;
-    const size_t shm = ((size_t)16 << KC) + progBytes + scratchBytes;
+    auto kern = k_fused_sweep<R, VAR, PULL>;
+    const size_t shm = ((size_t)16 << FUSED_KC) + progBytes + scratchBytes;
     static std::atomic<unsigned long long> attr_set_mask{ 0 }; // per device: the attribute is per-context
     if (!(attr_set_mask.load() & (1ULL << s->dev))) {
-        SV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-            (int)(((size_t)16 << KC) + (MINB >= 3 ? MAX_PROG_BYTES_3CTA : MAX_PROG_BYTES_2CTA))));
+        SV_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(((size_t)16 << FUSED_KC) + MAX_PROG_BYTES_2CTA)));
         attr_set_mask.fetch_or(1ULL << s->dev);
     }
-    const uint64_t maxGrid = (uint64_t)sm_count(s->dev) * MINB;
+    const uint64_t maxGrid = (uint64_t)sm_count(s->dev) * FUSED_MINB;
     const unsigned grid = (unsigned)std::min<uint64_t>(nTiles, maxGrid);
-    kern<<<grid, NT, shm, s->stream>>>(reinterpret_cast<typename Cx<R>::type*>(s->amps), dprog, progBytes, nTiles,
+    kern<<<grid, FUSED_NT, shm, s->stream>>>(reinterpret_cast<typename Cx<R>::type*>(s->amps), dprog, progBytes, nTiles,
         PULL ? s->pull : PullArgs{});
     SV_CUDA(cudaGetLastError());
     if (PULL) {
@@ -2455,150 +2365,13 @@ static int launch_sweep_v(State* s, const unsigned char* dprog, uint32_t progByt
     return B200SV_OK;
 }
 
-// tuning knobs (env B200SV_FUSED="RB,L32,L64"): register chunk bits per pass and the contiguous-run length (low tile bits)
-struct FusedKnobs {
-    int RB = 4;   // RB=4 (5 register qubits for fp32): more gates per pass than RB=3, still 2 CTAs per SM without spills
-    int L32 = 6;
-    int L64 = 6;
-    int RB64 = 4; // fp64, QFT-30 on an H100 (400 W): RB=4 / 2 CTAs per SM 109.5 ms vs RB=3 / 3 CTAs 114.9 ms per step
-    int bundle = 7; // bit 0: merge Hadamards on distinct register bits into one LAYER op; bit 1: DIAG phase groups;
-                    // bit 2: a LAYER stays open across ops that do not touch its qubits
-    int pf = 0;     // 1: L2 prefetch of the CTA's next tile during the passes
-    int minb64 = 3; // fp64 with RB64 = 3: resident CTAs per SM the kernel is compiled for (3: 80 registers, spills; 2: 128 registers)
-    int dlow = 1;   // first/last pass go straight HBM<->registers when at most this many of their register bits are chunk bits 0..2
-};
-static const FusedKnobs& knobs()
-{
-    static FusedKnobs k = [] {
-        FusedKnobs v;
-        const char* e = getenv("B200SV_FUSED");
-        if (e) {
-            int rb = 0, l32 = 0, l64 = 0, bn = 1, rb64 = 0, cp = 0, pf = 0, dlow = 1;
-            const int got = sscanf(e, "%d,%d,%d,%d,%d,%d,%d,%d", &rb, &l32, &l64, &bn, &rb64, &cp, &pf, &dlow);
-            if (got >= 6 && (cp == 2 || cp == 3)) {
-                v.minb64 = cp; // 6th field (formerly the constant-bank variant switch): CTAs/SM of the fp64 RB=3 kernel
-            }
-            if (got >= 8) {
-                v.dlow = dlow;
-            }
-            if (got >= 7) {
-                v.pf = pf;
-            }
-            if (got >= 4) {
-                v.bundle = bn;
-            }
-            if (got >= 5 && (rb64 == 3 || rb64 == 4)) {
-                v.RB64 = rb64;
-            }
-            if (got >= 1 && (rb == 3 || rb == 4)) {
-                v.RB = rb;
-            }
-            if (got >= 2 && l32 >= 5 && l32 <= 9) {
-                v.L32 = l32;
-            }
-            if (got >= 3 && l64 >= 4 && l64 <= 8) {
-                v.L64 = l64;
-            }
-        }
-        return v;
-    }();
-    return k;
-}
-template <typename R, int KC, int RB, int NT, int MINB>
+template <typename R>
 static int launch_sweep(State* s, const unsigned char* dprog, uint32_t progBytes, uint32_t scratchBytes, uint64_t nTiles, int var)
 {
     // var: 0 = light (STAGE / phase ops, Hadamard butterflies only), 1 = light + rotation stages, 2 = full (+ swap / general-matrix ops)
-    return var == 2 ? launch_sweep_v<R, KC, RB, NT, MINB, 2>(s, dprog, progBytes, scratchBytes, nTiles)
-                    : (var == 1 ? launch_sweep_v<R, KC, RB, NT, MINB, 1>(s, dprog, progBytes, scratchBytes, nTiles)
-                                : launch_sweep_v<R, KC, RB, NT, MINB, 0>(s, dprog, progBytes, scratchBytes, nTiles));
-}
-static int knob_prefetch() { return knobs().pf; }
-static int knob_plan_search()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_PLAN_SEARCH");
-        return e ? atoi(e) : 2;
-    }();
-    return v;
-}
-static int knob_direct_low() { return knobs().dlow; }
-static int knob_force_full()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_FORCE_FULL");
-        return e ? atoi(e) : 0;
-    }();
-    return v;
-}
-static int knob_lazy_diag()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_LAZY_DIAG");
-        return e ? atoi(e) : 1;
-    }();
-    return v;
-}
-static int knob_rewrite()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_REWRITE");
-        return e ? atoi(e) : 1;
-    }();
-    return v;
-}
-
-constexpr int FUSED_KC = 12;
-constexpr int FUSED_NT = 256;
-
-static int knob_plan_weight()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_PLAN_WEIGHT");
-        return e ? std::max(1, atoi(e)) : 1;
-    }();
-    return v;
-}
-static int knob_minb3()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_MINB3");
-        return e ? atoi(e) : 0;
-    }();
-    return v;
-}
-static int knob_rot()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_ROT");
-        return e ? atoi(e) : 1;
-    }();
-    return v;
-}
-static TileCfg state_cfg(int nq, int prec, bool light = false)
-{
-    const FusedKnobs& k = knobs();
-    (void)light;
-    TileCfg c = make_cfg(nq, prec, FUSED_KC, prec == 32 ? k.RB : k.RB64, prec == 32 ? k.L32 : k.L64, FUSED_NT);
-    c.bundle = k.bundle;
-    return c;
-}
-static bool flush_is_light(const std::vector<HostOp>& ops)
-{
-    for (const HostOp& h : ops) {
-        if (h.kind == OP_GENERAL || h.kind == OP_XSWAP) {
-            return false;
-        }
-    }
-    return true;
-}
-
-static int knob_pull_fused()
-{
-    static const int v = [] {
-        const char* e = getenv("B200SV_PULL_FUSED");
-        return e ? atoi(e) : 1;
-    }();
-    return v;
+    return var == 2 ? launch_sweep_v<R, 2>(s, dprog, progBytes, scratchBytes, nTiles)
+                    : (var == 1 ? launch_sweep_v<R, 1>(s, dprog, progBytes, scratchBytes, nTiles)
+                                : launch_sweep_v<R, 0>(s, dprog, progBytes, scratchBytes, nTiles));
 }
 
 int fused_flush(State* s, CarryReq* carry)
@@ -2613,7 +2386,7 @@ int fused_flush(State* s, CarryReq* carry)
     std::vector<HostOp> pending;
     uint64_t xtail = lower_queue(s->queue, pending);
     const size_t nGates = s->queue.size();
-    TileCfg cfg = state_cfg(s->nq, s->prec, flush_is_light(pending));
+    TileCfg cfg = make_cfg(s->nq, s->prec);
     cfg.virtMask = s->nVirt ? (((1ULL << s->nVirt) - 1ULL) << s->nq) : 0ULL;
     cfg.virtVal = s->virtVal;
     // build every sweep of this flush (nothing is launched before the whole flush is planned: a planner failure leaves the state as it was)
@@ -2621,8 +2394,8 @@ int fused_flush(State* s, CarryReq* carry)
     std::vector<Seg> segs;
     SV_TRY(plan_all(pending, cfg, s->prec, buf, segs, carry, &xtail));
     s->queue.clear();
-    // A pending re-page rides on the first sweep when there is one (RB = 4 instantiations only); otherwise it is a plain gather.
-    if (s->pullPending && (segs.empty() || cfg.RB != 4 || !knob_pull_fused())) {
+    // A pending re-page rides on the first sweep when there is one; otherwise it is a plain gather.
+    if (s->pullPending && segs.empty()) {
         SV_TRY(launch_pull_gather(s));
     }
     if (segs.empty()) {
@@ -2652,36 +2425,20 @@ int fused_flush(State* s, CarryReq* carry)
         const unsigned char* dp = ar->dev + segs[i].off;
         const uint32_t pb = (uint32_t)segs[i].bytes, sb = (uint32_t)segs[i].scratch;
         const DevSweep* dsw = reinterpret_cast<const DevSweep*>(buf.data() + segs[i].off);
-        const bool full = knob_force_full() || dsw->needFull != 0;
+        const bool full = dsw->needFull != 0;
         const int var = full ? 2 : (dsw->nRot ? 1 : 0);
         if (s->pullPending) {
-            // (i == 0) the re-page rides on this sweep: the full variant, two CTAs per SM
+            // (i == 0) the re-page rides on this sweep: the full variant
             if (s->prec == 32) {
-                SV_TRY((launch_sweep_v<float, FUSED_KC, 4, FUSED_NT, 2, 2, true>(s, dp, pb, sb, nTiles)));
+                SV_TRY((launch_sweep_v<float, 2, true>(s, dp, pb, sb, nTiles)));
             } else {
-                SV_TRY((launch_sweep_v<double, FUSED_KC, 4, FUSED_NT, 2, 2, true>(s, dp, pb, sb, nTiles)));
+                SV_TRY((launch_sweep_v<double, 2, true>(s, dp, pb, sb, nTiles)));
             }
             s->stats.pull_sweeps++;
         } else if (s->prec == 32) {
-            if (cfg.RB == 4 && var != 2 && knob_minb3() && (size_t)pb + (size_t)sb <= MAX_PROG_BYTES_3CTA) {
-                // light sweeps whose program fits beside three 64 KB tiles run three CTAs per SM (80 registers: the few spills sit
-                // in the per-pass setup, not in the op loop): 24 instead of 16 warps per SM hide more of the decode latency
-                SV_TRY((launch_sweep<float, FUSED_KC, 4, FUSED_NT, 3>(s, dp, pb, sb, nTiles, var)));
-            } else if (cfg.RB == 4) {
-                SV_TRY((launch_sweep<float, FUSED_KC, 4, FUSED_NT, 2>(s, dp, pb, sb, nTiles, var)));
-            } else {
-                SV_TRY((launch_sweep<float, FUSED_KC, 3, FUSED_NT, 3>(s, dp, pb, sb, nTiles, var)));
-            }
+            SV_TRY(launch_sweep<float>(s, dp, pb, sb, nTiles, var));
         } else {
-            if (cfg.RB == 4) {
-                SV_TRY((launch_sweep<double, FUSED_KC, 4, FUSED_NT, 2>(s, dp, pb, sb, nTiles, var)));
-            } else {
-                if (knobs().minb64 == 2) {
-                    SV_TRY((launch_sweep<double, FUSED_KC, 3, FUSED_NT, 2>(s, dp, pb, sb, nTiles, var)));
-                } else {
-                    SV_TRY((launch_sweep<double, FUSED_KC, 3, FUSED_NT, 3>(s, dp, pb, sb, nTiles, var)));
-                }
-            }
+            SV_TRY(launch_sweep<double>(s, dp, pb, sb, nTiles, var));
         }
         s->stats.kernel_launches++;
         s->stats.fused_sweeps++;
@@ -2718,12 +2475,7 @@ static void emu_exec_op(std::vector<EmuC<R>>& a, const DevOp<R>& op, uint32_t xs
     if (code & CODE_HAS_SB) {
         tp = (xsb & lmaskSb) == lvalSb;
     }
-    uint64_t em = tp ? (uint64_t)emask : 0ULL;
-    if (tp && NA > 32) {
-        uint32_t hi = 0;
-        memcpy(&hi, reinterpret_cast<const unsigned char*>(op.m) + 8, sizeof(hi));
-        em |= (uint64_t)hi << 32;
-    }
+    const uint32_t em = tp ? emask : 0U;
     const uint32_t c = code & 0xffU;
     auto had = [&](int J) {
         for (int e = 0; e < NA; ++e) {
@@ -2870,7 +2622,7 @@ static void emulate_sweep(const unsigned char* prog, EmuC<R>* psi, int nq, const
     const DevSweep& sw = *reinterpret_cast<const DevSweep*>(prog);
     const DevOp<R>* ops = reinterpret_cast<const DevOp<R>*>(prog + sizeof(DevSweep));
     const DevOuterPhase<R>* outer = reinterpret_cast<const DevOuterPhase<R>*>(prog + sw.outerOff);
-    const int APC = 1 << cfg.apcLog, NCH = 1 << cfg.RB, NA = NCH * APC, NT = cfg.NT;
+    const int APC = 1 << cfg.apcLog, NCH = 1 << FUSED_RB, NA = NCH * APC, NT = FUSED_NT;
     const int kc = sw.kc;
     const uint32_t nChunk = 1U << kc;
     const int lcb = sw.lowAmpBits - cfg.apcLog;
@@ -2886,7 +2638,7 @@ static void emulate_sweep(const unsigned char* prog, EmuC<R>* psi, int nq, const
         }
         rowOff[r] = off;
     }
-    const uint32_t nSub = nChunk >> cfg.RB;
+    const uint32_t nSub = nChunk >> FUSED_RB;
     const uint64_t nTiles = (1ULL << nq) >> cfg.kA;
     std::vector<EmuC<R>> tile((size_t)nChunk * APC); // indexed by swizzled chunk slot
     std::vector<R> tab((size_t)2 * std::max(1, sw.nSlots));
@@ -2998,7 +2750,7 @@ int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, voi
 {
     std::vector<HostOp> pending;
     uint64_t xtail = lower_queue(q, pending);
-    TileCfg cfg = state_cfg(n_qubits, precision, flush_is_light(pending));
+    TileCfg cfg = make_cfg(n_qubits, precision);
     cfg.virtMask = n_virtual ? (((1ULL << n_virtual) - 1ULL) << n_qubits) : 0ULL;
     cfg.virtVal = virt_value;
     std::vector<unsigned char> buf;
@@ -3007,7 +2759,7 @@ int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, voi
     if (!host_state) { // plan only (scripts/shard_sweep_count.py)
         return B200SV_OK;
     }
-    if (pull && (segs.empty() || cfg.RB != 4 || !knob_pull_fused())) { // launch_pull_gather on the device
+    if (pull && segs.empty()) { // launch_pull_gather on the device
         const uint64_t dim = 1ULL << n_qubits;
         for (uint64_t i = 0; i < dim; ++i) {
             if (precision == 32) {
@@ -3048,7 +2800,7 @@ int fused_plan_gates(int n_qubits, int precision, const std::vector<GateOp>& q, 
 {
     std::vector<HostOp> pending;
     (void)lower_queue(q, pending);
-    const TileCfg cfg = state_cfg(n_qubits, precision, flush_is_light(pending));
+    const TileCfg cfg = make_cfg(n_qubits, precision);
     int sweeps = 0, passes = 0, ops = 0;
     std::vector<unsigned char> buf;
     while (!pending.empty()) {
@@ -3063,68 +2815,6 @@ int fused_plan_gates(int n_qubits, int precision, const std::vector<GateOp>& q, 
     *n_sweeps = sweeps;
     *n_passes = passes;
     *n_ops = ops;
-    return B200SV_OK;
-}
-
-int fused_plan_dry_run(int n_qubits, int precision, int n_gates, const int* targets, const uint64_t* cmasks, const int* kinds,
-    int* n_sweeps, int* n_passes)
-{
-    std::vector<GateOp> q((size_t)n_gates);
-    for (int i = 0; i < n_gates; ++i) {
-        GateOp& g = q[i];
-        memset(&g, 0, sizeof(g));
-        g.target = targets[i];
-        g.cmask = cmasks[i];
-        g.cval = cmasks[i];
-        g.kind = kinds[i];
-        if (kinds[i] == 1) { // diagonal: T-like
-            g.m[0] = 1.0;
-            g.m[6] = 0.6;
-            g.m[7] = 0.8;
-        } else if (kinds[i] == 2) { // X-like
-            g.m[2] = 1.0;
-            g.m[4] = 1.0;
-        } else {
-            g.m[0] = 0.6;
-            g.m[2] = 0.8;
-            g.m[4] = 0.8;
-            g.m[6] = -0.6;
-            if (kinds[i] == 3) { // complex general, unitary: [[c, -e^{il} s], [e^{ip} s, e^{i(p+l)} c]], c = 0.8, s = 0.6, p = 0.3, l = 0.5
-                const double c = 0.8, sn = 0.6, ph = 0.3, la = 0.5;
-                g.m[0] = c;
-                g.m[1] = 0.0;
-                g.m[2] = -cos(la) * sn;
-                g.m[3] = -sin(la) * sn;
-                g.m[4] = cos(ph) * sn;
-                g.m[5] = sin(ph) * sn;
-                g.m[6] = cos(ph + la) * c;
-                g.m[7] = sin(ph + la) * c;
-            }
-            if (kinds[i] == 4) { // exact Hadamard
-                g.m[0] = g.m[2] = g.m[4] = 0.70710678118654752440;
-                g.m[6] = -g.m[0];
-            }
-        }
-    }
-    std::vector<HostOp> pending;
-    (void)lower_queue(q, pending);
-    const TileCfg cfg = state_cfg(n_qubits, precision, flush_is_light(pending));
-    int sweeps = 0, passes = 0;
-    std::vector<unsigned char> buf;
-    while (!pending.empty()) {
-        size_t bytes = 0, nops = 0;
-        int npass = 0;
-        buf.clear();
-        size_t scratch = 0;
-        SV_TRY(plan_and_encode(pending, cfg, precision, buf, &bytes, &scratch, &nops, &npass));
-        if (getenv("B200SV_FUSED_DEBUG")) {
-            fprintf(stderr, "  program %zu B + scratch %zu B%s\n", bytes, scratch, (bytes + scratch <= MAX_PROG_BYTES_3CTA) ? " (fits 3 CTAs/SM)" : "");
-        }
-        ++sweeps;
-        passes += npass;
-    }
-    *n_sweeps = sweeps;
-    *n_passes = passes;
     return B200SV_OK;
 }
 

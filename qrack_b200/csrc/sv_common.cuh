@@ -166,8 +166,6 @@ int launch_pull_gather(State* s); // the pending pull as a plain gather kernel (
 int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, void* host_state, const PullArgs* pull = nullptr,
     CarryReq* carry = nullptr, int n_virtual = 0, uint64_t virt_value = 0);
 int fused_plan_gates(int n_qubits, int precision, const std::vector<GateOp>& q, int* n_sweeps, int* n_passes, int* n_ops);
-int fused_plan_dry_run(int n_qubits, int precision, int n_gates, const int* targets, const uint64_t* cmasks, const int* kinds,
-    int* n_sweeps, int* n_passes);
 
 } // namespace b200sv
 

@@ -4,7 +4,6 @@
  (3) what the compiled reference returned for larger circuits (tests/golden/ref_*.npz),
  (4) size-independent properties at BASELINE.json's full sizes (28-30 qubits).
 Tolerances (north_star): max |delta amp| <= 1e-6 (fp32) / 1e-12 (fp64)."""
-import os
 import random
 
 import numpy as np
@@ -528,28 +527,21 @@ def test_memoised_marginals_follow_every_state_change(prec):
         assert abs(g2.Prob(q) - w) <= tol
 
 
-@pytest.mark.parametrize("env", [{"B200SV_MINB3": "1"}, {"B200SV_ROT": "0"}, {"B200SV_LAZY_DIAG": "0"}, {"B200SV_REWRITE": "0"},
-                                 {"B200SV_FORCE_FULL": "1"}, {"B200SV_FUSED": "3,6,6,7,3"}],
-                         ids=lambda e: ",".join("%s=%s" % kv for kv in e.items()))
-def test_scheduler_knobs_keep_parity_on_the_device(env):
-    """Every scheduler / kernel-variant switch (three CTAs per SM for small programs, rotation stages, lazy diagonals, the rewrite itself, the full kernel
-    variant, the RB=3 tile shape) must reproduce the oracle on the DEVICE kernels too (the library reads its knobs once per process,
-    hence the subprocess).  17-18 qubits: several tiles, high tile qubits, outer controls, thread-level members, several passes."""
-    import subprocess
-    import sys
-    code = (
-        "import sys, random; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-        "import numpy as np\n"
-        "from oracle.restate_engine import QEngineRestate\n"
-        "from qrack_b200 import QEngineCUDA, qscript\n"
-        "import util\n"
-        "for prec, n in ((32, 18), (64, 17)):\n"
-        "    text = (qscript.random_htcnot(n, 10, seed=3, timed=False) + qscript.quantum_volume(n, depth=4, seed=9, timed=False).split('\\n', 1)[1]\n"
-        "            + 'QFT 2 9\\nCCNOT 1 14 7\\nAntiCNOT 3 16\\nMCPhase 2 3 13 8 0.6 0.8 1 0\\nINC 5 1 9\\nXMask 3075\\nX 4\\nCZ 4 15\\n')\n"
-        "    want, _ = util.run_engine(text, QEngineRestate, prec)\n"
-        "    got, _ = util.run_engine(text, QEngineCUDA, prec)\n"
-        "    util.assert_states_close(got, want, prec, 'knobs')\n"
-        "print('ok')\n"
-    ) % (util.ROOT, os.path.join(util.ROOT, "tests"))
-    r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, **env), capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0 and "ok" in r.stdout, (r.stdout[-500:], r.stderr[-2000:])
+def test_fused_sweeps_keep_parity_on_the_device():
+    """Every variant of the fused sweep kernel reproduces the oracle on the device: Hadamard stages, rotation stages (the
+    quantum-volume layers) and the full variant (the controlled random unitary is a general-matrix op).  17-18 qubits:
+    several tiles, high tile qubits, outer controls, thread-level members, several passes."""
+    import math
+    rng = random.Random(12)
+    th, ph, la = (rng.uniform(-math.pi, math.pi) for _ in range(3))
+    c, s = math.cos(th / 2), math.sin(th / 2)
+    u = [c, -s * complex(math.cos(la), math.sin(la)), s * complex(math.cos(ph), math.sin(ph)),
+         c * complex(math.cos(ph + la), math.sin(ph + la))]
+    mcmtrx = "MCMtrx 2 6 11 0 %s\n" % " ".join("%.17g %.17g" % (complex(z).real, complex(z).imag) for z in u)
+    for prec, n in ((32, 18), (64, 17)):
+        text = (qscript.random_htcnot(n, 10, seed=3, timed=False) + qscript.quantum_volume(n, depth=4, seed=9, timed=False).split("\n", 1)[1]
+                + "QFT 2 9\nCCNOT 1 14 7\nAntiCNOT 3 16\nMCPhase 2 3 13 8 0.6 0.8 1 0\n" + mcmtrx
+                + "INC 5 1 9\nXMask 3075\nX 4\nCZ 4 15\n")
+        want, _ = util.run_engine(text, QEngineRestate, prec)
+        got, _ = util.run_engine(text, QEngineCUDA, prec)
+        util.assert_states_close(got, want, prec, "fused sweeps %d" % prec)
