@@ -155,7 +155,16 @@ def test_page_ops_and_shuffle(prec):
     qc = QEngineCUDA(n, 0, random.Random(1), 1.0, False, False, precision=prec)
     qc.CopyStateVec(qa)
     assert np.array_equal(qc.GetQuantumState(), ea)
-    assert abs(qc.SumSqrDiff(qa)) < 1e-5 or True
+    # SumSqrDiff = 1 - |<this|other>|^2 (state.cpp:2109-2165), on normalised states with a known overlap
+    u = (a0 / np.linalg.norm(a0)).astype(dt)
+    v = (u + 0.5 * b0 / np.linalg.norm(b0)).astype(np.complex128)
+    v = (v / np.linalg.norm(v)).astype(dt)
+    qc.SetQuantumState(u)
+    qa.SetQuantumState(v)
+    want = 1.0 - abs(np.vdot(u.astype(np.complex128), v.astype(np.complex128))) ** 2
+    assert 0.1 < want < 0.9
+    assert abs(qc.SumSqrDiff(qa) - want) <= util.PROB_TOL[prec]
+    assert abs(qc.SumSqrDiff(qc.Clone())) <= util.PROB_TOL[prec]
 
 
 @pytest.mark.parametrize("prec", [32, 64])
