@@ -1727,8 +1727,8 @@ int b200sv_ipc_release(int device, void* ptr)
 int b200sv_exchange_scatter(b200sv_t s, int k, const int* victim_bits, int rank, void* const* dst_pages)
 {
     SV_ENTER(s);
-    if (k < 1 || k > 8 || !victim_bits || !dst_pages) {
-        return einval("exchange_scatter: bad arguments");
+    if (k < 1 || k > 8 || !victim_bits || !dst_pages || rank < 0 || rank >= (1 << k)) {
+        return einval("exchange_scatter: bad arguments (1 <= k <= 8, 0 <= rank < 2^k)");
     }
     if (!s->amps) {
         return einval("exchange_scatter: zero state");

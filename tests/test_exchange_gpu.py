@@ -10,6 +10,7 @@ import pytest
 
 from qrack_b200 import _abi
 
+import npref
 import util
 from test_fused_emulation import _random_gate_arrays
 
@@ -23,21 +24,6 @@ def _pages(lib, n, nbytes):
         _abi.check(lib, lib.b200sv_alloc_page(0, nbytes, ctypes.byref(p)))
         out.append(p.value)
     return out
-
-
-def _expected_exchange(pages, k, vb, nl, rank):
-    idx = np.arange(1 << nl, dtype=np.uint64)
-    src_rank = np.zeros(1 << nl, dtype=np.int64)
-    for b in range(k):
-        src_rank |= (((idx >> np.uint64(vb[b])) & np.uint64(1)).astype(np.int64) << b)
-    vmask = sum(1 << b for b in vb)
-    dep = sum((1 << vb[b]) for b in range(k) if (rank >> b) & 1)
-    src_idx = (idx & np.uint64(~vmask & ((1 << nl) - 1))) | np.uint64(dep)
-    want = np.empty(1 << nl, dtype=pages[0].dtype)
-    for r in range(len(pages)):
-        sel = src_rank == r
-        want[sel] = pages[r][src_idx[sel]]
-    return want
 
 
 @pytest.mark.parametrize("prec", [32, 64])
@@ -80,7 +66,7 @@ def test_exchange_pull_and_push_on_one_device(prec, k, nl, n_gates):
                 eng[r].be.apply_gates(g, o1, o2, pm, mats)
         got = [eng[r].be.get_state() for r in range(W)]
         for r in range(W):
-            want = _expected_exchange(host, k, vb, nl, r)
+            want = npref.exchange(host, k, vb, r)
             assert np.array_equal(pushed[r], want), ("push", r, vb)
             st = eng[r].be.stats()
             if g:

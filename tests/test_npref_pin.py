@@ -217,3 +217,83 @@ def test_gate_families_reach_every_fused_op_kind(capfd, monkeypatch):
     for token in ("STAGE(", "PH2.", "PHGEN", "XSWAP.", "GEN_U.", "GEN_P."):
         assert token in text, "no %s op in the lowered families" % token
     assert ", rotation 0)" not in seen["rotation"].splitlines()[0], seen["rotation"].splitlines()[0]
+
+
+# ---- QAlu maps and the re-page --------------------------------------------------------------------------------------
+
+def check_alu_cases(n, prec, psi, cases):
+    for name, args in cases:
+        o = oracle(n, prec, psi)
+        getattr(o.be, "alu_" + name)(*args)
+        got = o.be.get_state()
+        want = getattr(npref, name)(psi, *args)
+        assert np.array_equal(got, want.astype(got.dtype)), "%s%r at %dq: %d amplitudes differ" % (
+            name, args[:7], n, int(np.sum(got != want)))
+
+
+@pytest.mark.parametrize("prec", [32, 64])
+@pytest.mark.parametrize("n", list(range(6, 15)))
+def test_qalu_reference_matches_the_oracle(n, prec):
+    """Every QAlu map of npref on the edge grid of the device test, bit for bit against the oracle restatement (itself pinned
+    to the compiled reference by the alu_* golden fixtures): index maps and sign flips of the amplitudes, nothing rounds."""
+    psi = dense(np.random.default_rng(40 + n), n, prec)
+    check_alu_cases(n, prec, psi, npref.alu_grid(n))
+
+
+@pytest.mark.parametrize("prec", [32, 64])
+@pytest.mark.parametrize("n", [12, 19])
+def test_wide_qalu_reference_matches_the_oracle(n, prec):
+    """The wide-register calls of the device test, 2- and 3-byte table entries among them (19 qubits hold a 17-bit value
+    register with its index bit and carry)."""
+    psi = dense(np.random.default_rng(60 + n), n, prec)
+    check_alu_cases(n, prec, psi, npref.alu_wide(n))
+
+
+def test_forward_maps_must_be_injective():
+    """A forward map that sends two sources to one destination has no defined result: the reference refuses it."""
+    psi = dense(np.random.default_rng(3), 6, 64)
+    with pytest.raises(AssertionError, match="not injective"):
+        npref.muldiv(psi, 0, 16, 0, 3, 3, 0)                # 16 * 4 wraps past the 6 bits of register and carry to 0
+    with pytest.raises(AssertionError, match="not injective"):
+        npref.muldiv(psi, 0, 0, 0, 3, 3, 0)
+    with pytest.raises(AssertionError, match="not injective"):
+        npref.hash(psi, 0, 2, bytes([0, 1, 1, 2]))
+
+
+def test_exchange_reference_is_a_rank_permutation():
+    """Re-paging twice with the same victim bits is the identity, and every amplitude of every page lands exactly once."""
+    nl, k, vb = 7, 2, [5, 1]
+    pages = [np.arange(r << nl, (r + 1) << nl).astype(np.complex128) for r in range(1 << k)]
+    new = [npref.exchange(pages, k, vb, r) for r in range(1 << k)]
+    assert np.array_equal(np.sort(np.concatenate(new).real), np.arange(4 << nl))
+    for r in range(1 << k):
+        assert np.array_equal(npref.exchange(new, k, vb, r), pages[r])
+        # element i: source rank = (bit 5, bit 1) of i, index = i with those bits := this rank's bits
+        i = 0b1100010
+        assert new[r][i] == pages[3][(i & ~0b100010) | ((r & 1) << 5) | ((r >> 1) << 1)]
+
+
+def first_sweep_direct_flags(n, prec, gates, capfd, monkeypatch):
+    monkeypatch.setenv("B200SV_FUSED_DEBUG", "1")
+    capfd.readouterr()
+    k, o1, o2, pm, m8 = npref.pack_gates(gates)
+    ns, npass, nops = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+    rc = _abi.load().b200sv_plan_gates(n, prec, k, o1, o2, pm, m8, ctypes.byref(ns), ctypes.byref(npass), ctypes.byref(nops))
+    assert rc == _abi.B200SV_OK
+    err = capfd.readouterr().err
+    first = next(line for line in err.splitlines() if line.strip().startswith("sweep:"))
+    return int(first.split("directIn")[1].split(",")[0]), first
+
+
+@pytest.mark.parametrize("prec", [32, 64])
+@pytest.mark.parametrize("n", [13, 16])
+def test_pull_gate_lists_take_both_first_pass_paths(n, prec, capfd, monkeypatch):
+    """The first sweep of a flush carries a pending pull re-page.  Its first pass reads the source pages either through the
+    staged tile copy (stage_in_pull: directIn 0) or with direct per-thread loads (pull_src in the pass: directIn 1); the
+    planner decides per sweep.  The two gate lists per family of the device pull test must reach one each."""
+    for family in ("light", "rotation", "full"):
+        staged, direct = npref.pull_gate_lists(family, n, prec)
+        d, line = first_sweep_direct_flags(n, prec, staged, capfd, monkeypatch)
+        assert d == 0, (family, "staged", line)
+        d, line = first_sweep_direct_flags(n, prec, direct, capfd, monkeypatch)
+        assert d == 1, (family, "direct", line)
