@@ -39,6 +39,16 @@ protected:
     /// OR of 2^control; throws std::invalid_argument like ThrowIfQbIdArrayIsBad (common/qrack_functions.hpp)
     uint64_t CtrlMask(const std::vector<bitLenInt>& controls, const char* what) const;
 
+    /// the sum-form weights as uint64 (false: a perm, the offset or the largest weight does not fit — the base class loops)
+    bool BitsWeights(const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset,
+        std::vector<int>& b, std::vector<uint64_t>& p, uint64_t& off) const;
+    /// (S0, S1, S2) of b200sv_moments_bits / _floats after the doNormalize step
+    void Moments(const std::vector<int>& b, const std::vector<uint64_t>& p, uint64_t off, double center, double* out);
+    void MomentsFloats(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights, double* out);
+    /// drops PauliI as the reference's loop does (some survive it and count as PauliZ); false when a qubit is out of bounds or
+    /// repeated (the base class then throws what it throws)
+    bool PauliMasks(std::vector<bitLenInt>& bits, const std::vector<Pauli>& paulis, uint64_t& x, uint64_t& z) const;
+
 public:
     /// 1 / OclMemDenom of device memory is the most a single state vector should take (test/benchmarks_main.cpp:288)
     static const bitCapIntOcl OclMemDenom = 3U;
@@ -116,6 +126,17 @@ public:
     bitCapInt HighestProbAll(); // device arg-max; the QInterface default asks ProbAll() for every permutation
     real1_f FirstNonzeroPhase() override { return IsZeroAmplitude() ? ZERO_R1_F : QInterface::FirstNonzeroPhase(); }
     real1_f GetExpectation(bitLenInt valueStart, bitLenInt valueLength) override;
+    // The QInterface defaults ask ProbAll(i) — one device round trip — for every basis state (qinterface.cpp:478-800); here a
+    // k >= 2 query is one read-only sweep (two for VarianceBitsFactorized).  ExpectationBitsAll / VarianceBitsAll, the
+    // *UnitaryAll and the *Rdm forms reach these through QInterface's own virtual calls.
+    real1_f ExpectationBitsFactorized(
+        const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset = ZERO_BCI) override;
+    real1_f VarianceBitsFactorized(
+        const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset = ZERO_BCI) override;
+    real1_f ExpectationFloatsFactorized(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights) override;
+    real1_f VarianceFloatsFactorized(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights) override;
+    real1_f ExpectationPauliAll(std::vector<bitLenInt> bits, std::vector<Pauli> paulis) override;
+    real1_f VariancePauliAll(std::vector<bitLenInt> bits, std::vector<Pauli> paulis) override;
 
     // ---- structure ----
     using QEngine::Compose;

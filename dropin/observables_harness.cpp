@@ -1,0 +1,140 @@
+// observables_harness.cpp — replays a qscript circuit of U / CNOT gates followed by the observable queries of QInterface on a
+// QEngine built by the reference's factory, and prints one result line per query in the qscript result format
+// ("<op> <value>", as qrack_b200/qscript.py appends them).  Compiled against the reference's own QEngineCPU it produces the
+// expected values of tests/golden/ref_observables_12q.*.npz (tests/golden/make_observables.py); compiled by dropin/Makefile
+// against the drop-in, `--engine cuda` runs the same queries through QEngineCUDA's overrides.
+//
+//   observables_harness <script> [--engine cpu|cuda] [--dump FILE]
+//
+// Ops (tokens as in qrack_b200/qscript.py; <cs> = count then qubits):
+//   qubits N | U q theta phi lambda | CNOT c t
+//   ExpectationBitsAll|VarianceBitsAll <cs> offset
+//   ExpectationBitsFactorized|VarianceBitsFactorized <cs> offset perm0 .. perm{2n-1}
+//   ExpectationFloatsFactorized|VarianceFloatsFactorized <cs> weight0 .. weight{2n-1}
+//   ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}
+//   ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..
+#include "qfactory.hpp"
+
+#include <cstdio>
+#include <cstdlib>
+#include <fstream>
+#include <sstream>
+#include <string>
+#include <vector>
+
+using namespace Qrack;
+
+int main(int argc, char** argv)
+{
+    if (argc < 2) {
+        fprintf(stderr, "usage: %s <script> [--engine cpu|cuda] [--dump FILE]\n", argv[0]);
+        return 2;
+    }
+    std::string engine = "cpu", dump;
+    for (int a = 2; a + 1 < argc; a += 2) {
+        const std::string s = argv[a];
+        if (s == "--engine") {
+            engine = argv[a + 1];
+        } else if (s == "--dump") {
+            dump = argv[a + 1];
+        }
+    }
+    std::ifstream in(argv[1]);
+    if (!in) {
+        fprintf(stderr, "cannot open %s\n", argv[1]);
+        return 2;
+    }
+    QInterfacePtr q;
+    std::string line;
+    while (std::getline(in, line)) {
+        const size_t h = line.find('#');
+        if (h != std::string::npos) {
+            line.resize(h);
+        }
+        std::istringstream ts(line);
+        std::string op;
+        if (!(ts >> op)) {
+            continue;
+        }
+        if (op == "qubits") {
+            int n;
+            ts >> n;
+            qrack_rand_gen_ptr rng = std::make_shared<qrack_rand_gen>();
+            rng->seed(20250921U);
+            q = CreateQuantumInterface((engine == "cuda") ? QINTERFACE_CUDA : QINTERFACE_CPU, (bitLenInt)n, ZERO_BCI, rng,
+                ONE_CMPLX, false, false, false, -1, false);
+            continue;
+        }
+        if (op == "U") {
+            int t;
+            double th, ph, la;
+            ts >> t >> th >> ph >> la;
+            q->U((bitLenInt)t, (real1_f)th, (real1_f)ph, (real1_f)la);
+            continue;
+        }
+        if (op == "CNOT") {
+            int c, t;
+            ts >> c >> t;
+            q->CNOT((bitLenInt)c, (bitLenInt)t);
+            continue;
+        }
+        int k;
+        ts >> k;
+        std::vector<bitLenInt> bits(k);
+        for (int i = 0; i < k; ++i) {
+            int b;
+            ts >> b;
+            bits[i] = (bitLenInt)b;
+        }
+        double r;
+        if (op == "ExpectationBitsAll" || op == "VarianceBitsAll") {
+            unsigned long long off;
+            ts >> off;
+            r = (op[0] == 'E') ? q->ExpectationBitsAll(bits, bitCapInt((uint64_t)off))
+                               : q->VarianceBitsAll(bits, bitCapInt((uint64_t)off));
+        } else if (op == "ExpectationBitsFactorized" || op == "VarianceBitsFactorized") {
+            unsigned long long off, v;
+            ts >> off;
+            std::vector<bitCapInt> perms;
+            while (ts >> v) {
+                perms.push_back(bitCapInt((uint64_t)v));
+            }
+            r = (op[0] == 'E') ? q->ExpectationBitsFactorized(bits, perms, bitCapInt((uint64_t)off))
+                               : q->VarianceBitsFactorized(bits, perms, bitCapInt((uint64_t)off));
+        } else if (op == "ExpectationFloatsFactorized" || op == "VarianceFloatsFactorized" || op == "ExpectationUnitaryAll" ||
+            op == "VarianceUnitaryAll") {
+            double v;
+            std::vector<real1_f> w;
+            while (ts >> v) {
+                w.push_back((real1_f)v);
+            }
+            if (op == "ExpectationFloatsFactorized") {
+                r = q->ExpectationFloatsFactorized(bits, w);
+            } else if (op == "VarianceFloatsFactorized") {
+                r = q->VarianceFloatsFactorized(bits, w);
+            } else if (op == "ExpectationUnitaryAll") {
+                r = q->ExpectationUnitaryAll(bits, w);
+            } else {
+                r = q->VarianceUnitaryAll(bits, w);
+            }
+        } else if (op == "ExpectationPauliAll" || op == "VariancePauliAll") {
+            int v;
+            std::vector<Pauli> ps;
+            while (ts >> v) {
+                ps.push_back((Pauli)v);
+            }
+            r = (op[0] == 'E') ? q->ExpectationPauliAll(bits, ps) : q->VariancePauliAll(bits, ps);
+        } else {
+            fprintf(stderr, "unknown op '%s'\n", op.c_str());
+            return 2;
+        }
+        printf("%s %.17g\n", op.c_str(), r);
+    }
+    if (!dump.empty() && q) {
+        std::vector<complex> st((size_t)(bitCapIntOcl)q->GetMaxQPower());
+        q->GetQuantumState(st.data());
+        std::ofstream out(dump, std::ios::binary);
+        out.write((const char*)st.data(), st.size() * sizeof(complex));
+    }
+    return 0;
+}

@@ -747,6 +747,224 @@ real1_f QEngineCUDA::GetExpectation(bitLenInt valueStart, bitLenInt valueLength)
     return (tot > 0) ? (real1_f)(avg / tot) : (real1_f)avg;
 }
 
+// ---- observables (reference src/qinterface/qinterface.cpp:542-806): same checks and messages, same k = 0 / k = 1 branches
+// (the base class's, over Prob), and one read-only sweep for k >= 2 --------------------------------------------------------
+
+bool QEngineCUDA::BitsWeights(const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset,
+    std::vector<int>& b, std::vector<uint64_t>& p, uint64_t& off) const
+{
+    const bitCapInt max64 = bitCapInt(~(uint64_t)0U);
+    if (bi_compare(offset, max64) > 0) {
+        return false;
+    }
+    off = (uint64_t)offset;
+    uint64_t top = off;
+    b.resize(bits.size());
+    p.resize(bits.size() << 1U);
+    for (size_t i = 0U; i < bits.size(); ++i) {
+        b[i] = (int)bits[i];
+        for (size_t e = 0U; e < 2U; ++e) {
+            const bitCapInt& v = perms[(i << 1U) | e];
+            if (bi_compare(v, max64) > 0) {
+                return false;
+            }
+            p[(i << 1U) | e] = (uint64_t)v;
+        }
+        const uint64_t m = std::max(p[i << 1U], p[(i << 1U) | 1U]);
+        if (m > ~top) {
+            return false;
+        }
+        top += m;
+    }
+    return true;
+}
+
+void QEngineCUDA::Moments(const std::vector<int>& b, const std::vector<uint64_t>& p, uint64_t off, double center, double* out)
+{
+    if (doNormalize) {
+        NormalizeState();
+    }
+    Check(b200sv_moments_bits(sv, (int)b.size(), b.data(), p.data(), off, center, out));
+}
+
+void QEngineCUDA::MomentsFloats(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights, double* out)
+{
+    if (doNormalize) {
+        NormalizeState();
+    }
+    std::vector<int> b(bits.begin(), bits.end());
+    std::vector<double> w(weights.begin(), weights.begin() + (bits.size() << 1U));
+    Check(b200sv_moments_floats(sv, (int)b.size(), b.data(), w.data(), 0.0, out));
+}
+
+real1_f QEngineCUDA::ExpectationBitsFactorized(
+    const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset)
+{
+    if (perms.size() < (bits.size() << 1U)) {
+        throw std::invalid_argument(
+            "QInterface::ExpectationBitsFactorized() must supply at least twice as many 'perms' as bits!");
+    }
+    ThrowIfQbIdArrayIsBad(bits, qubitCount,
+        "QInterface::ExpectationBitsFactorized() parameter qubits vector values must be within allocated qubit "
+        "bounds!");
+    std::vector<int> b;
+    std::vector<uint64_t> p;
+    uint64_t off = 0U;
+    if ((bits.size() < 2U) || !BitsWeights(bits, perms, offset, b, p, off)) {
+        return QEngine::ExpectationBitsFactorized(bits, perms, offset);
+    }
+    double m[3];
+    Moments(b, p, off, 0.0, m);
+    return (real1_f)m[1];
+}
+
+real1_f QEngineCUDA::VarianceBitsFactorized(
+    const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset)
+{
+    if (perms.size() < (bits.size() << 1U)) {
+        throw std::invalid_argument(
+            "QInterface::VarianceBitsFactorized() must supply at least twice as many 'perms' as bits!");
+    }
+    ThrowIfQbIdArrayIsBad(bits, qubitCount,
+        "QInterface::VarianceBitsFactorized() parameter qubits vector values must be within allocated qubit "
+        "bounds!");
+    std::vector<int> b;
+    std::vector<uint64_t> p;
+    uint64_t off = 0U;
+    if ((bits.size() < 2U) || !BitsWeights(bits, perms, offset, b, p, off)) {
+        return QEngine::VarianceBitsFactorized(bits, perms, offset);
+    }
+    const real1_f mean = ExpectationBitsFactorized(bits, perms, offset);
+    // a second sweep centred on the mean: sum p (w - mean)^2 without the cancellation of E[w^2] - E[w]^2
+    double m[3];
+    Moments(b, p, off, (double)mean, m);
+    return (real1_f)m[2];
+}
+
+real1_f QEngineCUDA::ExpectationFloatsFactorized(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights)
+{
+    if (weights.size() < (bits.size() << 1U)) {
+        throw std::invalid_argument(
+            "QInterface::ExpectationFloatsFactorized() must supply at least twice as many weights as bits!");
+    }
+    ThrowIfQbIdArrayIsBad(bits, qubitCount,
+        "QInterface::ExpectationFloatsFactorized() parameter qubits vector values must be within allocated qubit "
+        "bounds!");
+    if (bits.size() < 2U) {
+        return QEngine::ExpectationFloatsFactorized(bits, weights);
+    }
+    double m[3];
+    MomentsFloats(bits, weights, m);
+    return (real1_f)m[1];
+}
+
+real1_f QEngineCUDA::VarianceFloatsFactorized(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights)
+{
+    if (weights.size() < (bits.size() << 1U)) {
+        throw std::invalid_argument(
+            "QInterface::VarianceFloatsFactorized() must supply at least twice as many weights as bits!");
+    }
+    ThrowIfQbIdArrayIsBad(bits, qubitCount,
+        "QInterface::VarianceFloatsFactorized() parameter qubits vector values must be within allocated qubit "
+        "bounds!");
+    if (bits.size() < 2U) {
+        return QEngine::VarianceFloatsFactorized(bits, weights);
+    }
+    double m[3];
+    MomentsFloats(bits, weights, m);
+    // the reference sums p (w - mean) UNSQUARED for k >= 2 (qinterface.cpp:653) = mean (1 - S0); kept for parity with
+    // QEngineCPU (its 1-bit branch squares; the true variance is S2 centred on the mean)
+    const real1_f mean = (real1_f)m[1];
+    return (real1_f)(m[1] - (double)mean * m[0]);
+}
+
+bool QEngineCUDA::PauliMasks(std::vector<bitLenInt>& bits, const std::vector<Pauli>& paulis, uint64_t& x, uint64_t& z) const
+{
+    if (paulis.size() < bits.size()) {
+        return false;
+    }
+    // the PauliI-dropping loop of qinterface.cpp:719-726 as written: it re-reads bits.size() after each erase, so some PauliI
+    // entries survive it, and those then get the weights (1, -1) without a basis gate — they count as PauliZ
+    std::vector<Pauli> ps(paulis.begin(), paulis.begin() + bits.size());
+    for (size_t i = 0U; i < bits.size(); ++i) {
+        const size_t j = bits.size() - (i + 1U);
+        if (ps[j] == PauliI) {
+            bits.erase(bits.begin() + j);
+            ps.erase(ps.begin() + j);
+        }
+    }
+    x = z = 0U;
+    for (size_t i = 0U; i < bits.size(); ++i) {
+        if (bits[i] >= qubitCount) {
+            return false;
+        }
+        const uint64_t pw = pow2Ocl(bits[i]);
+        if ((x | z) & pw) {
+            return false;
+        }
+        // include/pauli.hpp: X = 1, Z = 2, Y = 3
+        if (ps[i] == PauliX || ps[i] == PauliY) {
+            x |= pw;
+        }
+        if (ps[i] != PauliX) {
+            z |= pw;
+        }
+    }
+    return true;
+}
+
+// ExpectationPauliAll / VariancePauliAll (qinterface.cpp:659-769) rotate each X / Y qubit into the Z basis, run the Floats query
+// with weights (1, -1) and rotate back.  b200sv_expectation_pauli returns S0 = sum |psi|^2 and E = <psi|P|psi> without
+// touching the state; in the rotated basis Prob(bits[0]) of the 1-bit branch is (S0 - E) / 2 and the k >= 2 sum is E.
+real1_f QEngineCUDA::ExpectationPauliAll(std::vector<bitLenInt> bits, std::vector<Pauli> paulis)
+{
+    std::vector<bitLenInt> kept = bits;
+    uint64_t x = 0U, z = 0U;
+    if (!PauliMasks(kept, paulis, x, z)) {
+        return QEngine::ExpectationPauliAll(bits, paulis);
+    }
+    if (kept.empty()) {
+        return ONE_R1_F;
+    }
+    if (doNormalize) {
+        NormalizeState();
+    }
+    double o[2];
+    Check(b200sv_expectation_pauli(sv, x, z, o));
+    if (kept.size() == 1U) {
+        const real1_f prob = clampProb((real1_f)((o[0] - o[1]) / 2));
+        return (ONE_R1_F - prob) - prob;
+    }
+    return (real1_f)o[1];
+}
+
+real1_f QEngineCUDA::VariancePauliAll(std::vector<bitLenInt> bits, std::vector<Pauli> paulis)
+{
+    std::vector<bitLenInt> kept = bits;
+    uint64_t x = 0U, z = 0U;
+    if (!PauliMasks(kept, paulis, x, z)) {
+        return QEngine::VariancePauliAll(bits, paulis);
+    }
+    if (kept.empty()) {
+        return ONE_R1_F;
+    }
+    if (doNormalize) {
+        NormalizeState();
+    }
+    double o[2];
+    Check(b200sv_expectation_pauli(sv, x, z, o));
+    if (kept.size() == 1U) {
+        const real1_f prob = clampProb((real1_f)((o[0] - o[1]) / 2));
+        const real1_f mean = (ONE_R1_F - prob) - prob;
+        const real1_f var0 = ONE_R1_F - mean;
+        const real1_f var1 = -ONE_R1_F - mean;
+        return var0 * var0 * (ONE_R1_F - prob) + var1 * var1 * prob;
+    }
+    // VarianceFloatsFactorized's unsquared k >= 2 sum with weights (1, -1): E - E S0
+    const real1_f mean = (real1_f)o[1];
+    return (real1_f)(o[1] - (double)mean * o[0]);
+}
+
 // ---- structure (reference state.cpp:1271-1748, utility.cpp:54-68) --------------------------------------------------
 
 bitLenInt QEngineCUDA::Compose(QEngineCUDAPtr toCopy) { return Compose(toCopy, qubitCount); }

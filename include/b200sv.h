@@ -124,8 +124,33 @@ int b200sv_norm(b200sv_t s, double norm_thresh, double* out);
 int b200sv_normalize(b200sv_t s, double nrm, double norm_thresh, double phase_arg);
 /* <a|b> (SumSqrDiff :2109-2165) */
 int b200sv_inner(b200sv_t a, b200sv_t b, double* re, double* im);
-/* sum_i |psi[i]|^2 * ((i >> start) & (2^length - 1))  (GetExpectation, utility.cpp) */
+/* sum_i |psi[i]|^2 * ((i >> start) & (2^length - 1))  (GetExpectation, utility.cpp); the moments sweep below with
+ * perms (0, 2^p) on qubit start + p */
 int b200sv_expectation(b200sv_t s, int start, int length, double* out);
+
+/* ---- observables: one read-only sweep each instead of the 2^n ProbAll(i) calls of the QInterface defaults
+ * (src/qinterface/qinterface.cpp:478-800).  Queued gates are flushed first; the memoised Prob marginals stay valid and
+ * the state is not written.  The zero state returns zeros without a launch.  Every term is accumulated in double.
+ *
+ * Weighted moments: out[0] = sum_i |psi_i|^2, out[1] = sum_i |psi_i|^2 (w_i - center), out[2] = sum_i |psi_i|^2 (w_i - center)^2,
+ * with w_i depending on the bits of i at the k distinct qubits bits[0..k-1]:
+ *   bits form   w_i = offset + sum_p perms[2p + bit(i, bits[p])], summed in uint64 (exact) and converted to double once —
+ *               the retIndex of ExpectationBitsFactorized / VarianceBitsFactorized (:542-618);
+ *   floats form w_i = prod_p weights[2p + bit(i, bits[p])] — ExpectationFloatsFactorized (:771-806) and
+ *               VarianceFloatsFactorized (:620-657).
+ * k = 0 gives w = offset (bits form) or 1 (floats form).  out[1] with center 0 is the expectation; out[2] with center = that
+ * expectation is the true variance (a second sweep, which avoids the cancellation of E[w^2] - E[w]^2).  Note that the
+ * reference's VarianceFloatsFactorized for k >= 2 returns the UNSQUARED sum_i p_i (w_i - mean) (:653) = mean (1 - out[0]);
+ * its 1-bit branch squares.  B200SV_EINVAL when k < 0, bits / the table / out is NULL where needed, a qubit is outside
+ * [0, n) or repeated, or (bits form) offset + sum_p max(perms[2p], perms[2p + 1]) exceeds 2^64 - 1. */
+int b200sv_moments_bits(b200sv_t s, int k, const int* bits, const uint64_t* perms, uint64_t offset, double center,
+    double* out);
+int b200sv_moments_floats(b200sv_t s, int k, const int* bits, const double* weights, double center, double* out);
+/* Pauli string P with X on x & ~z, Y on x & z, Z on z & ~x: out[0] = sum |psi|^2, out[1] = <psi|P|psi>
+ * = sum_j conj(psi[j ^ x]) i^popcount(x & z) (-1)^popcount(j & z) psi[j], every pair (j, j ^ x) read once.  What
+ * ExpectationPauliAll (:715-769) computes by applying H / IS.H basis gates, running the Floats sweep with weights (1, -1)
+ * and undoing the gates — here without writing the state.  B200SV_EINVAL when out is NULL or a mask is >= 2^n. */
+int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, double* out);
 /* index of the largest |psi|^2 (HighestProbAll :1995-2024) */
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm);
 /* smallest index i with |psi[i]|^2 > REAL1_EPSILON and cumulative cum = sum_{j<=i} |psi[j]|^2 > rnd or 1 - cum <= FP_NORM_EPSILON,

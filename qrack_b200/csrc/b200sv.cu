@@ -739,16 +739,6 @@ __global__ void __launch_bounds__(256) k_inner(const typename Cx<R>::type* __res
     block_atomic_add(im, out + 1);
 }
 
-template <typename R>
-__global__ void __launch_bounds__(256) k_expectation(const typename Cx<R>::type* __restrict__ psi, uint64_t n, int start,
-    uint64_t lenMask, double* out)
-{
-    typedef typename Cx<R>::type C;
-    double acc = 0;
-    for_amps<R>(psi, n, [&](uint64_t i, C a) { acc += (double)cnorm(a) * (double)((i >> start) & lenMask); });
-    block_atomic_add(acc, out);
-}
-
 template <typename R, typename RO>
 __global__ void __launch_bounds__(256) k_probs(const typename Cx<R>::type* __restrict__ psi, uint64_t n, RO* out)
 {
@@ -1480,6 +1470,7 @@ static int flush_queue(State* s)
 } // namespace b200sv
 
 #include "alu_kernels.cuh"
+#include "observables.cuh"
 
 using namespace b200sv;
 
@@ -2977,17 +2968,87 @@ int b200sv_expectation(b200sv_t s, int start, int length, double* out)
         *out = 0;
         return B200SV_OK;
     }
-    const uint64_t n = s->dim();
-    const unsigned grid = stream_grid(s->dev, n, 256);
-    SV_CUDA(cudaMemsetAsync(s->d_scratch, 0, sizeof(double), s->stream));
-    const uint64_t lm = (1ULL << length) - 1U;
-    DISPATCH_PREC(s, (k_expectation<float><<<grid, 256, 0, s->stream>>>((const float2*)s->amps, n, start, lm, s->d_scratch)),
-        (k_expectation<double><<<grid, 256, 0, s->stream>>>((const double2*)s->amps, n, start, lm, s->d_scratch)));
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
-    SV_TRY(read_scratch(s, 1));
-    *out = s->h_scratch[0];
+    // the sum form with perms (0, 2^p) on qubit start + p
+    std::vector<int> bits(length);
+    std::vector<uint64_t> perms(2 * (size_t)length);
+    for (int p = 0; p < length; ++p) {
+        bits[p] = start + p;
+        perms[2 * p] = 0U;
+        perms[2 * p + 1] = 1ULL << p;
+    }
+    double m[3];
+    SV_TRY(launch_moments(s, false, length, bits.data(), perms.data(), nullptr, 0U, 0.0, m));
+    *out = m[1];
     return B200SV_OK;
+}
+
+// argument checks shared by the two moments entries (before anything touches the state)
+static int moments_args(const State* s, int k, const int* bits, const void* table, const double* out)
+{
+    if (k < 0 || !out || (k > 0 && (!bits || !table))) {
+        return einval("moments: k < 0 or a NULL argument");
+    }
+    uint64_t seen = 0U;
+    for (int p = 0; p < k; ++p) {
+        if (bits[p] < 0 || bits[p] >= s->nq) {
+            return einval("moments: qubit index out of bounds");
+        }
+        if ((seen >> bits[p]) & 1U) {
+            return einval("moments: repeated qubit");
+        }
+        seen |= 1ULL << bits[p];
+    }
+    return B200SV_OK;
+}
+
+int b200sv_moments_bits(b200sv_t s, int k, const int* bits, const uint64_t* perms, uint64_t offset, double center, double* out)
+{
+    SV_ENTER_RO(s);
+    SV_TRY(moments_args(s, k, bits, perms, out));
+    // the largest weight must fit: offset + sum_p max(perms[2p], perms[2p + 1]) <= 2^64 - 1
+    uint64_t top = offset;
+    for (int p = 0; p < k; ++p) {
+        const uint64_t m = std::max(perms[2 * p], perms[2 * p + 1]);
+        if (m > ~top) {
+            return einval("moments_bits: offset + sum of the largest perms exceeds 2^64 - 1");
+        }
+        top += m;
+    }
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        out[0] = out[1] = out[2] = 0;
+        return B200SV_OK;
+    }
+    return launch_moments(s, false, k, bits, perms, nullptr, offset, center, out);
+}
+
+int b200sv_moments_floats(b200sv_t s, int k, const int* bits, const double* weights, double center, double* out)
+{
+    SV_ENTER_RO(s);
+    SV_TRY(moments_args(s, k, bits, weights, out));
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        out[0] = out[1] = out[2] = 0;
+        return B200SV_OK;
+    }
+    return launch_moments(s, true, k, bits, nullptr, weights, 0U, center, out);
+}
+
+int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, double* out)
+{
+    SV_ENTER_RO(s);
+    if (!out) {
+        return einval("null out pointer");
+    }
+    if (x_mask >= s->dim() || z_mask >= s->dim()) {
+        return einval("expectation_pauli: mask out-of-bounds!");
+    }
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        out[0] = out[1] = 0;
+        return B200SV_OK;
+    }
+    return launch_pauli(s, x_mask, z_mask, out);
 }
 
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm)

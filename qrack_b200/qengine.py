@@ -974,6 +974,202 @@ class QEngineHost:
             src |= ((idx >> p) & 1) << order.index(b)
         return asc[src]
 
+    # ---- observables ------------------------------------------------------------------------------------------
+    # The QInterface defaults (src/qinterface/qinterface.cpp:478-800) loop over all 2^n basis states and ask ProbAll(i) for each.
+    # Here every k >= 2 query is one read-only device sweep (b200sv_moments_bits / _floats / b200sv_expectation_pauli), a
+    # sum-form variance two; the k = 0 and k = 1 branches are the reference's own (1, and the Prob(bits[0]) formula).
+    _U64 = (1 << 64) - 1
+
+    def _obs_check(self, bits, table, what: str, tname: str):  # the checks of :546-553 and their messages
+        if len(table) < 2 * len(bits):
+            raise ValueError("QInterface::%s() must supply at least twice as many %s as bits!" % (what, tname))
+        msg = "QInterface::%s() parameter qubits vector values must be within allocated qubit bounds!" % what
+        seen = set()
+        for b in bits:
+            if b < 0 or b >= self.qubitCount:
+                raise ValueError(msg)
+            if b in seen:
+                raise ValueError(msg + " (Found duplicate qubit indices!)")
+            seen.add(b)
+
+    def _bits_weights(self, bits, perms, offset, mean: Optional[float]) -> float:
+        """k >= 2 sum form with a perm, offset or largest weight beyond uint64: the reference's loop over ProbAll (:560-576,
+        :600-616) in Python integers, so nothing changes there."""
+        tot = 0.0
+        for lcv in range(self.maxQPower):
+            w = offset + sum(perms[2 * p + ((lcv >> b) & 1)] for p, b in enumerate(bits))
+            pr = self.ProbAll(lcv)
+            tot += float(w) * pr if mean is None else (float(w) - mean) ** 2 * pr
+        return self._r(tot)
+
+    def _bits_fit(self, perms, offset) -> bool:
+        top = offset + sum(max(perms[2 * p], perms[2 * p + 1]) for p in range(len(perms) // 2))
+        return 0 <= offset and all(0 <= v <= self._U64 for v in perms) and top <= self._U64
+
+    def ExpectationBitsFactorized(self, bits, perms, offset: int = 0) -> float:  # qinterface.cpp:542-577
+        bits, perms, offset = [int(b) for b in bits], [int(v) for v in perms], int(offset)
+        self._obs_check(bits, perms, "ExpectationBitsFactorized", "'perms'")
+        return self._expectation_bits(bits, perms, offset)
+
+    def _expectation_bits(self, bits, perms, offset) -> float:
+        if not bits:
+            return 1.0
+        if len(bits) == 1:
+            pr = self.Prob(bits[0])
+            return self._r(float(perms[0] + offset) * (1.0 - pr) + float(perms[1] + offset) * pr)
+        perms = perms[:2 * len(bits)]
+        if not self._bits_fit(perms, offset):
+            return self._bits_weights(bits, perms, offset, None)
+        if self.doNormalize:
+            self.NormalizeState()
+        return self._r(self.be.moments_bits(bits, perms, offset, 0.0)[1])
+
+    def VarianceBitsFactorized(self, bits, perms, offset: int = 0) -> float:  # qinterface.cpp:579-618
+        bits, perms, offset = [int(b) for b in bits], [int(v) for v in perms], int(offset)
+        self._obs_check(bits, perms, "VarianceBitsFactorized", "'perms'")
+        if not bits:
+            return 1.0
+        mean = self._expectation_bits(bits, perms, offset)
+        if len(bits) == 1:
+            pr = self.Prob(bits[0])
+            d0, d1 = self._r(float(perms[0] + offset) - mean), self._r(float(perms[1] + offset) - mean)
+            return self._r(d0 * d0 * (1.0 - pr) + d1 * d1 * pr)
+        perms = perms[:2 * len(bits)]
+        if not self._bits_fit(perms, offset):
+            return self._bits_weights(bits, perms, offset, mean)
+        # a second sweep centred on the mean: no cancellation of E[w^2] - E[w]^2
+        return self._r(self.be.moments_bits(bits, perms, offset, mean)[2])
+
+    def ExpectationBitsAll(self, bits, offset: int = 0) -> float:  # ExpVarBitsAll, qinterface.hpp:210-219
+        return self.ExpectationBitsFactorized(bits, self._bits_all_perms(len(bits)), offset)
+
+    def VarianceBitsAll(self, bits, offset: int = 0) -> float:
+        return self.VarianceBitsFactorized(bits, self._bits_all_perms(len(bits)), offset)
+
+    @staticmethod
+    def _bits_all_perms(k: int) -> List[int]:
+        perms = []
+        for i in range(k):
+            perms += [0, 1 << i]
+        return perms
+
+    def _floats_sweep(self, bits, weights):
+        if self.doNormalize:
+            self.NormalizeState()
+        return self.be.moments_floats(bits, weights[:2 * len(bits)], 0.0)
+
+    def ExpectationFloatsFactorized(self, bits, weights) -> float:  # qinterface.cpp:771-806
+        bits, weights = [int(b) for b in bits], [self._r(w) for w in weights]
+        self._obs_check(bits, weights, "ExpectationFloatsFactorized", "weights")
+        if not bits:
+            return 1.0
+        if len(bits) == 1:
+            pr = self.Prob(bits[0])
+            return self._r(weights[0] * (1.0 - pr) + weights[1] * pr)
+        return self._r(self._floats_sweep(bits, weights)[1])
+
+    def VarianceFloatsFactorized(self, bits, weights) -> float:  # qinterface.cpp:620-657
+        bits, weights = [int(b) for b in bits], [self._r(w) for w in weights]
+        self._obs_check(bits, weights, "VarianceFloatsFactorized", "weights")
+        if not bits:
+            return 1.0
+        if len(bits) == 1:
+            pr = self.Prob(bits[0])
+            mean = self._r(weights[0] * (1.0 - pr) + weights[1] * pr)
+            v0, v1 = self._r(weights[0] - mean), self._r(weights[1] - mean)
+            return self._r(v0 * v0 * (1.0 - pr) + v1 * v1 * pr)
+        s0, s1, _ = self._floats_sweep(bits, weights)
+        # the reference sums p_i (w_i - mean) UNSQUARED here (:653); parity with it, not the variance (that is s2 centred on
+        # the mean)
+        mean = self._r(s1)
+        return self._r(s1 - mean * s0)
+
+    @staticmethod
+    def _drop_pauli_i(bits, paulis):
+        """the PauliI-dropping loop of qinterface.cpp:663-670 / 719-726 as written: it re-reads bits.size() after each erase,
+        so some PauliI entries survive it — and then weigh like PauliZ (weights (1, -1), no basis gate)"""
+        bits, paulis = [int(b) for b in bits], [int(p) for p in paulis]
+        i = 0
+        while i < len(bits):
+            j = len(bits) - (i + 1)
+            if paulis[j] == 0:
+                del bits[j]
+                del paulis[j]
+            i += 1
+        return bits, paulis
+
+    def _pauli(self, bits, paulis):
+        """(kept bits, S0, E) for the string left by _drop_pauli_i, with X = 1, Z = 2, Y = 3 (include/pauli.hpp) and a
+        surviving I as Z"""
+        kept, x, z = [], 0, 0
+        for b, p in zip(*self._drop_pauli_i(bits, paulis)):
+            if p == 0:
+                p = 2
+            self._check_qubit(b, "ExpectationPauliAll")
+            if b in kept:
+                raise ValueError("ExpectationPauliAll: duplicate qubit")
+            kept.append(b)
+            x |= (p & 1) << b
+            z |= ((p >> 1) & 1) << b
+        if not kept:
+            return kept, 0.0, 0.0
+        if self.doNormalize:
+            self.NormalizeState()
+        s0, e = self.be.expectation_pauli(x, z)
+        return kept, s0, e
+
+    def ExpectationPauliAll(self, bits, paulis) -> float:  # qinterface.cpp:715-769
+        kept, s0, e = self._pauli(bits, paulis)
+        if not kept:
+            return 1.0
+        if len(kept) == 1:
+            # Prob of the rotated qubit is (S0 - E) / 2; weights (1, -1)
+            pr = self.clampProb(self._r((s0 - e) / 2.0))
+            return self._r((1.0 - pr) - pr)
+        return self._r(e)
+
+    def VariancePauliAll(self, bits, paulis) -> float:  # qinterface.cpp:659-713
+        kept, s0, e = self._pauli(bits, paulis)
+        if not kept:
+            return 1.0
+        if len(kept) == 1:
+            pr = self.clampProb(self._r((s0 - e) / 2.0))
+            mean = self._r((1.0 - pr) - pr)
+            v0, v1 = self._r(1.0 - mean), self._r(-1.0 - mean)
+            return self._r(v0 * v0 * (1.0 - pr) + v1 * v1 * pr)
+        # VarianceFloatsFactorized's unsquared sum with weights (1, -1): E - E * S0
+        mean = self._r(e)
+        return self._r(e - mean * s0)
+
+    def _exp_var_unitary(self, isExp: bool, bits, basisOps, eigenVals) -> float:
+        """QInterface::ExpVarUnitaryAll (qinterface.cpp:478-540): the inverse basis gates, the Floats query, the gates again.
+        basisOps = 3 U angles per qubit (theta, phi, lambda) or one 2x2 matrix per qubit."""
+        bits = [int(b) for b in bits]
+        if not bits:
+            return 1.0
+        eigenVals = list(eigenVals) if eigenVals else [1.0, -1.0] * len(bits)
+        mtrx = len(basisOps) > 0 and hasattr(basisOps[0], "__len__")
+        for i, b in enumerate(bits):
+            if mtrx:
+                m = [complex(v) for v in basisOps[i]]
+                det = 1.0 / (m[0] * m[3] - m[1] * m[2])  # inv2x2, src/common/functions.cpp:204-211
+                self.Mtrx([det * m[3], det * -m[1], det * -m[2], det * m[0]], b)
+            else:
+                self.U(b, -basisOps[3 * i], -basisOps[3 * i + 1], -basisOps[3 * i + 2])
+        r = self.ExpectationFloatsFactorized(bits, eigenVals) if isExp else self.VarianceFloatsFactorized(bits, eigenVals)
+        for i, b in enumerate(bits):
+            if mtrx:
+                self.Mtrx([complex(v) for v in basisOps[i]], b)
+            else:
+                self.U(b, basisOps[3 * i], basisOps[3 * i + 1], basisOps[3 * i + 2])
+        return r
+
+    def ExpectationUnitaryAll(self, bits, basisOps, eigenVals=()) -> float:
+        return self._exp_var_unitary(True, bits, basisOps, eigenVals)
+
+    def VarianceUnitaryAll(self, bits, basisOps, eigenVals=()) -> float:
+        return self._exp_var_unitary(False, bits, basisOps, eigenVals)
+
     def MultiShotMeasureMask(self, qPowers: Sequence[int], shots: int) -> dict:
         """QEngine::MultiShotMeasureMask (src/qengine/qengine.cpp:542-576): `shots` samples of the listed qubits without
         collapse, as {outcome: count} with qPowers[p] -> outcome bit p.  Few measured qubits: one histogram sweep
@@ -1441,6 +1637,32 @@ class _CudaBackend:
 
     def expectation(self, start, length) -> float:
         return self._scalar(self.lib.b200sv_expectation, start, length)
+
+    def _moments(self, fn, bits, table, ctype, *args):
+        import ctypes
+        k = len(bits)
+        b = (ctypes.c_int * max(k, 1))(*bits)
+        t = (ctype * max(2 * k, 1))(*table[:2 * k])
+        out = (ctypes.c_double * 3)()
+        self._ck(fn(self.h, k, b, t, *args, out))
+        return out[0], out[1], out[2]
+
+    def moments_bits(self, bits, perms, offset, center):
+        """(S0, S1, S2) of the sum-form weight (b200sv_moments_bits)"""
+        import ctypes
+        return self._moments(self.lib.b200sv_moments_bits, bits, perms, ctypes.c_uint64, int(offset), float(center))
+
+    def moments_floats(self, bits, weights, center):
+        """(S0, S1, S2) of the product-form weight (b200sv_moments_floats)"""
+        import ctypes
+        return self._moments(self.lib.b200sv_moments_floats, bits, weights, ctypes.c_double, float(center))
+
+    def expectation_pauli(self, x_mask, z_mask):
+        """(sum |psi|^2, <psi|P|psi>) of the Pauli string (x_mask, z_mask) (b200sv_expectation_pauli)"""
+        import ctypes
+        out = (ctypes.c_double * 2)()
+        self._ck(self.lib.b200sv_expectation_pauli(self.h, x_mask, z_mask, out))
+        return out[0], out[1]
 
     def highest_prob(self) -> int:
         import ctypes

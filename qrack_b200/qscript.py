@@ -30,6 +30,11 @@ Grammar (tokens are whitespace separated; ``<m8>`` = 8 reals = 4 complex row-maj
   queries (each appends one line to the results):
     Prob q   ProbAll perm   ProbReg start length perm   ProbMask mask perm   ProbParity mask
     CProb c t   ACProb c t   GetAmplitude perm   SumSqrDiff OTHER   Norm
+    ExpectationBitsAll|VarianceBitsAll <cs> offset
+    ExpectationBitsFactorized|VarianceBitsFactorized <cs> offset perm0 .. perm{2n-1}
+    ExpectationFloatsFactorized|VarianceFloatsFactorized <cs> weight0 .. weight{2n-1}
+    ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}        (0 = I, 1 = X, 2 = Z, 3 = Y: include/pauli.hpp)
+    ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..  (the U3 form of ExpVarUnitaryAll)
 """
 from __future__ import annotations
 
@@ -39,6 +44,9 @@ from typing import Callable, Dict, Iterable, List, Sequence, Tuple
 
 QUERY_OPS = {
     "Prob", "ProbAll", "ProbReg", "ProbMask", "ProbParity", "CProb", "ACProb", "GetAmplitude", "SumSqrDiff", "Norm",
+    "ExpectationBitsAll", "VarianceBitsAll", "ExpectationBitsFactorized", "VarianceBitsFactorized",
+    "ExpectationFloatsFactorized", "VarianceFloatsFactorized", "ExpectationPauliAll", "VariancePauliAll",
+    "ExpectationUnitaryAll", "VarianceUnitaryAll",
 }
 
 
@@ -208,6 +216,18 @@ def run(text: str, make_reg: Callable[[int, int], object]) -> Tuple[Dict[int, ob
         elif op == "Norm":
             q.UpdateRunningNorm()
             results.append((op, (q.GetRunningNorm(),)))
+        elif op in ("ExpectationBitsAll", "VarianceBitsAll"):
+            c, p = _qubits(t, 1)
+            results.append((op, (getattr(q, op)(c, int(t[p])),)))
+        elif op in ("ExpectationBitsFactorized", "VarianceBitsFactorized"):
+            c, p = _qubits(t, 1)
+            results.append((op, (getattr(q, op)(c, [int(x) for x in t[p + 1:]], int(t[p])),)))
+        elif op in ("ExpectationFloatsFactorized", "VarianceFloatsFactorized", "ExpectationUnitaryAll", "VarianceUnitaryAll"):
+            c, p = _qubits(t, 1)
+            results.append((op, (getattr(q, op)(c, [float(x) for x in t[p:]]),)))
+        elif op in ("ExpectationPauliAll", "VariancePauliAll"):
+            c, p = _qubits(t, 1)
+            results.append((op, (getattr(q, op)(c, [int(x) for x in t[p:]]),)))
         else:
             raise ValueError("qscript: unknown op %r" % op)
     return regs, results

@@ -546,7 +546,8 @@ class _ShardedBackend:
             res = res[np.arange(res.size, dtype=np.int64) ^ flip]   # logical outcome = stored outcome ^ inversions on the mask
         return res
 
-    _UNSUPPORTED = ("collapse_parity", "uniform_parity_rz", "uniformly_controlled", "inner", "expectation", "compose", "decompose",
+    _UNSUPPORTED = ("collapse_parity", "uniform_parity_rz", "uniformly_controlled", "inner", "expectation", "moments_bits",
+                    "moments_floats", "expectation_pauli", "compose", "decompose",
                     "dispose_perm", "get_page", "set_page", "copy_page", "shuffle", "copy_state", "clone")
 
     def __getattr__(self, name):
