@@ -137,6 +137,9 @@ public:
     real1_f VarianceFloatsFactorized(const std::vector<bitLenInt>& bits, const std::vector<real1_f>& weights) override;
     real1_f ExpectationPauliAll(std::vector<bitLenInt> bits, std::vector<Pauli> paulis) override;
     real1_f VariancePauliAll(std::vector<bitLenInt> bits, std::vector<Pauli> paulis) override;
+    // The QInterface default asks GetAmplitude 2^n (1 + 2^k) times (qinterface.cpp:886-944); here it is one read-only sweep.
+    // An out-of-range or repeated qubit throws std::invalid_argument; k > B200SV_RDM_MAX_QUBITS goes to the base class.
+    void GetReducedDensityMatrix(const std::vector<bitLenInt>& qubits, complex* outputState) override;
 
     // ---- structure ----
     using QEngine::Compose;

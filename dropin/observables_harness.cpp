@@ -1,6 +1,6 @@
 // observables_harness.cpp — replays a qscript circuit of U / CNOT gates followed by the observable queries of QInterface on a
 // QEngine built by the reference's factory, and prints one result line per query in the qscript result format
-// ("<op> <value>", as qrack_b200/qscript.py appends them).  Compiled against the reference's own QEngineCPU it produces the
+// ("<op> <value> ..", as qrack_b200/qscript.py appends them).  Compiled against the reference's own QEngineCPU it produces the
 // expected values of tests/golden/ref_observables_12q.*.npz (tests/golden/make_observables.py); compiled by dropin/Makefile
 // against the drop-in, `--engine cuda` runs the same queries through QEngineCUDA's overrides.
 //
@@ -13,6 +13,7 @@
 //   ExpectationFloatsFactorized|VarianceFloatsFactorized <cs> weight0 .. weight{2n-1}
 //   ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}
 //   ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..
+//   GetReducedDensityMatrix <cs>          (prints the 2 4^n values of rho row-major, interleaved re / im)
 #include "qfactory.hpp"
 
 #include <cstdio>
@@ -85,6 +86,17 @@ int main(int argc, char** argv)
             int b;
             ts >> b;
             bits[i] = (bitLenInt)b;
+        }
+        if (op == "GetReducedDensityMatrix") {
+            const size_t dim = (size_t)1U << k;
+            std::vector<complex> rho(dim * dim);
+            q->GetReducedDensityMatrix(bits, rho.data());
+            printf("%s", op.c_str());
+            for (const complex& z : rho) {
+                printf(" %.17g %.17g", (double)real(z), (double)imag(z));
+            }
+            printf("\n");
+            continue;
         }
         double r;
         if (op == "ExpectationBitsAll" || op == "VarianceBitsAll") {

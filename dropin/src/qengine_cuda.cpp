@@ -965,6 +965,32 @@ real1_f QEngineCUDA::VariancePauliAll(std::vector<bitLenInt> bits, std::vector<P
     return (real1_f)(o[1] - (double)mean * o[0]);
 }
 
+void QEngineCUDA::GetReducedDensityMatrix(const std::vector<bitLenInt>& qubits, complex* outputState)
+{
+    std::vector<bool> seen(qubitCount, false);
+    for (const bitLenInt q : qubits) {
+        if (q >= qubitCount) {
+            throw std::invalid_argument("QEngineCUDA::GetReducedDensityMatrix qubit index out of bounds!");
+        }
+        if (seen[q]) {
+            throw std::invalid_argument("QEngineCUDA::GetReducedDensityMatrix repeated qubit index!");
+        }
+        seen[q] = true;
+    }
+    if (qubits.size() > B200SV_RDM_MAX_QUBITS) {
+        QInterface::GetReducedDensityMatrix(qubits, outputState);
+        return;
+    }
+    // like the base class (GetAmplitude, state.cpp:193) this does not normalise
+    const size_t dim = (size_t)1U << qubits.size();
+    std::vector<int> q(qubits.begin(), qubits.end());
+    std::vector<double> rho(2U * dim * dim);
+    Check(b200sv_reduced_density_matrix(sv, (int)q.size(), q.data(), rho.data()));
+    for (size_t i = 0U; i < dim * dim; ++i) {
+        outputState[i] = complex((real1)rho[2U * i], (real1)rho[2U * i + 1U]);
+    }
+}
+
 // ---- structure (reference state.cpp:1271-1748, utility.cpp:54-68) --------------------------------------------------
 
 bitLenInt QEngineCUDA::Compose(QEngineCUDAPtr toCopy) { return Compose(toCopy, qubitCount); }

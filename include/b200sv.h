@@ -151,6 +151,14 @@ int b200sv_moments_floats(b200sv_t s, int k, const int* bits, const double* weig
  * ExpectationPauliAll (:715-769) computes by applying H / IS.H basis gates, running the Floats sweep with weights (1, -1)
  * and undoing the gates — here without writing the state.  B200SV_EINVAL when out is NULL or a mask is >= 2^n. */
 int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, double* out);
+/* Reduced density matrix on the k qubits qubits[0..k-1] (GetReducedDensityMatrix, qinterface.cpp:886-944):
+ * out[2 (i 2^k + j)] + i out[2 (i 2^k + j) + 1] = sum_e psi[i, e] conj(psi[j, e]), where bit p of i and j is
+ * qubit qubits[p] (the order given, not sorted) and e runs over the other qubits.  Not normalised.
+ * Read-only; the zero state gives zeros.  B200SV_EINVAL when k < 0, k > B200SV_RDM_MAX_QUBITS (14), k > n,
+ * qubits (k > 0) or out is NULL, a qubit is outside [0, n) or repeated.  B200SV_ENOMEM when the device buffer
+ * cannot be had. */
+#define B200SV_RDM_MAX_QUBITS 14
+int b200sv_reduced_density_matrix(b200sv_t s, int k, const int* qubits, double* out);
 /* index of the largest |psi|^2 (HighestProbAll :1995-2024) */
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm);
 /* smallest index i with |psi[i]|^2 > REAL1_EPSILON and cumulative cum = sum_{j<=i} |psi[j]|^2 > rnd or 1 - cum <= FP_NORM_EPSILON,

@@ -1471,6 +1471,7 @@ static int flush_queue(State* s)
 
 #include "alu_kernels.cuh"
 #include "observables.cuh"
+#include "rdm.cuh"
 
 using namespace b200sv;
 
@@ -3049,6 +3050,48 @@ int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, doubl
         return B200SV_OK;
     }
     return launch_pauli(s, x_mask, z_mask, out);
+}
+
+int b200sv_reduced_density_matrix(b200sv_t s, int k, const int* qubits, double* out)
+{
+    SV_ENTER_RO(s);
+    if (k < 0 || k > B200SV_RDM_MAX_QUBITS || k > s->nq || !out || (k > 0 && !qubits)) {
+        return einval("reduced_density_matrix: k out of range or a NULL argument");
+    }
+    uint64_t seen = 0U;
+    for (int p = 0; p < k; ++p) {
+        if (qubits[p] < 0 || qubits[p] >= s->nq) {
+            return einval("reduced_density_matrix: qubit index out of bounds");
+        }
+        if ((seen >> qubits[p]) & 1U) {
+            return einval("reduced_density_matrix: repeated qubit");
+        }
+        seen |= 1ULL << qubits[p];
+    }
+    SV_TRY(flush_queue(s));
+    const size_t words = (size_t)2 << (2 * k);
+    if (!s->amps) {
+        std::fill(out, out + words, 0.0);
+        return B200SV_OK;
+    }
+    if (s->nq == 0) {
+        // one amplitude, smaller than a 16-byte chunk: rho = |psi_0|^2
+        double a[2] = {0.0, 0.0};
+        if (s->prec == 32) {
+            float f[2];
+            SV_CUDA(cudaMemcpyAsync(f, s->amps, sizeof(f), cudaMemcpyDeviceToHost, s->stream));
+            SV_CUDA(cudaStreamSynchronize(s->stream));
+            a[0] = f[0];
+            a[1] = f[1];
+        } else {
+            SV_CUDA(cudaMemcpyAsync(a, s->amps, sizeof(a), cudaMemcpyDeviceToHost, s->stream));
+            SV_CUDA(cudaStreamSynchronize(s->stream));
+        }
+        out[0] = a[0] * a[0] + a[1] * a[1];
+        out[1] = 0.0;
+        return B200SV_OK;
+    }
+    return launch_rdm(s, k, qubits, out);
 }
 
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm)

@@ -1170,6 +1170,25 @@ class QEngineHost:
     def VarianceUnitaryAll(self, bits, basisOps, eigenVals=()) -> float:
         return self._exp_var_unitary(False, bits, basisOps, eigenVals)
 
+    # ---- reduced density matrix -------------------------------------------------------------------------------
+    RDM_MAX_QUBITS = 14  # B200SV_RDM_MAX_QUBITS
+
+    def GetReducedDensityMatrix(self, qubits) -> np.ndarray:
+        """QInterface::GetReducedDensityMatrix (src/qinterface/qinterface.cpp:886-944) as one read-only device sweep
+        (b200sv_reduced_density_matrix) instead of 2^n (1 + 2^k) GetAmplitude calls: rho[i, j] = sum_e psi[i, e] conj(psi[j, e]),
+        bit p of i and j being qubit qubits[p] in the order given, e running over the other qubits.  Shape (2^k, 2^k), in the
+        engine's complex type.  Like the reference (which reads through GetAmplitude, state.cpp:193) it does not normalise, so
+        the trace is sum |psi|^2 whatever doNormalize says.  A qubit out of range or repeated, or more than 14 qubits, raise
+        ValueError (the reference indexes out of bounds there)."""
+        qubits = [int(q) for q in qubits]
+        if len(qubits) > self.RDM_MAX_QUBITS:
+            raise ValueError("GetReducedDensityMatrix: at most %d qubits" % self.RDM_MAX_QUBITS)
+        for q in qubits:
+            self._check_qubit(q, "GetReducedDensityMatrix")
+        if len(set(qubits)) != len(qubits):
+            raise ValueError("GetReducedDensityMatrix: repeated qubit")
+        return self.be.reduced_density_matrix(qubits).astype(self.cplx)
+
     def MultiShotMeasureMask(self, qPowers: Sequence[int], shots: int) -> dict:
         """QEngine::MultiShotMeasureMask (src/qengine/qengine.cpp:542-576): `shots` samples of the listed qubits without
         collapse, as {outcome: count} with qPowers[p] -> outcome bit p.  Few measured qubits: one histogram sweep
@@ -1663,6 +1682,15 @@ class _CudaBackend:
         out = (ctypes.c_double * 2)()
         self._ck(self.lib.b200sv_expectation_pauli(self.h, x_mask, z_mask, out))
         return out[0], out[1]
+
+    def reduced_density_matrix(self, qubits) -> np.ndarray:
+        """rho on the listed qubits, complex128 of shape (2^k, 2^k) (b200sv_reduced_density_matrix)"""
+        import ctypes
+        k = len(qubits)
+        q = (ctypes.c_int * max(k, 1))(*qubits)
+        out = np.empty(2 << (2 * k), dtype=np.float64)
+        self._ck(self.lib.b200sv_reduced_density_matrix(self.h, k, q, out.ctypes.data_as(ctypes.POINTER(ctypes.c_double))))
+        return out.view(np.complex128).reshape(1 << k, 1 << k)
 
     def highest_prob(self) -> int:
         import ctypes

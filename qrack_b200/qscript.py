@@ -35,6 +35,7 @@ Grammar (tokens are whitespace separated; ``<m8>`` = 8 reals = 4 complex row-maj
     ExpectationFloatsFactorized|VarianceFloatsFactorized <cs> weight0 .. weight{2n-1}
     ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}        (0 = I, 1 = X, 2 = Z, 3 = Y: include/pauli.hpp)
     ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..  (the U3 form of ExpVarUnitaryAll)
+    GetReducedDensityMatrix <cs>      (the 2 4^n values of rho row-major, interleaved re / im; bit p of a row is qubit p of <cs>)
 """
 from __future__ import annotations
 
@@ -46,7 +47,7 @@ QUERY_OPS = {
     "Prob", "ProbAll", "ProbReg", "ProbMask", "ProbParity", "CProb", "ACProb", "GetAmplitude", "SumSqrDiff", "Norm",
     "ExpectationBitsAll", "VarianceBitsAll", "ExpectationBitsFactorized", "VarianceBitsFactorized",
     "ExpectationFloatsFactorized", "VarianceFloatsFactorized", "ExpectationPauliAll", "VariancePauliAll",
-    "ExpectationUnitaryAll", "VarianceUnitaryAll",
+    "ExpectationUnitaryAll", "VarianceUnitaryAll", "GetReducedDensityMatrix",
 }
 
 
@@ -228,6 +229,13 @@ def run(text: str, make_reg: Callable[[int, int], object]) -> Tuple[Dict[int, ob
         elif op in ("ExpectationPauliAll", "VariancePauliAll"):
             c, p = _qubits(t, 1)
             results.append((op, (getattr(q, op)(c, [int(x) for x in t[p:]]),)))
+        elif op == "GetReducedDensityMatrix":
+            c, _ = _qubits(t, 1)
+            vals = []
+            for row in q.GetReducedDensityMatrix(c):
+                for z in row:
+                    vals += [float(z.real), float(z.imag)]
+            results.append((op, tuple(vals)))
         else:
             raise ValueError("qscript: unknown op %r" % op)
     return regs, results
