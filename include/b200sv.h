@@ -204,25 +204,6 @@ int b200sv_exchange_pull(b200sv_t s, int k, const int* victim_bits, int rank, vo
 
 /* ---- queue / fusion control ---- */
 int b200sv_flush(b200sv_t s);  /* launch everything queued; does not wait */
-/* Rank bits of a sharded register as VIRTUAL qubits n_qubits .. n_qubits+k-1 of this page's engine: index bits the page does not
- * hold, with the constant value `rank` here.  Gates passed to b200sv_apply_gates may then use them as controls, and diagonal
- * gates as their own qubit; the predicate is folded when a sweep is encoded (an op that cannot fire on this rank emits nothing),
- * and what b200sv_flush_carry hands back keeps them — so that it stays valid after an exchange has turned them into real qubits
- * of the page (a gate specialised for this rank by the caller would not).  k = 0 switches them off.
- * (Reference: QPager keeps the page index outside its engines and specialises every gate per page on the host — meta-controlled
- * gates select pages, src/qpager.cpp:452-593; there is no counterpart of a gate list that survives a re-page.) */
-int b200sv_set_rank_bits(b200sv_t s, int k, uint64_t rank);
-/* b200sv_flush that leaves the under-filled TAIL of the window un-executed: trailing fused sweeps that would hold fewer than
- * `min_ops` lowered ops are not launched; everything not executed is handed back, in program order, as single-target gates in
- * the layout of b200sv_apply_gates (n_out <= cap of them) for the caller to submit again later — e.g. after a page exchange,
- * relabelled, where they merge into the dense first sweeps of the next window instead of costing nearly empty passes over the
- * state (each sweep streams the whole page whatever it holds).  No op handed back is a non-diagonal gate on a qubit of
- * `must_mask` (the qubits about to leave the page); min_ops = 0 is b200sv_flush.  On a sharded register every rank must call it
- * with the same queue and arguments (b200sv_set_rank_bits makes the queues equal): the choice of what is handed back is made on
- * the symbolic op list and is then the same everywhere.  (Reference: QPager executes gate by gate, swap-compute-swap around each
- * gate on a paged qubit, src/qpager.cpp:425-432 — there is no window to cut.) */
-int b200sv_flush_carry(b200sv_t s, int min_ops, uint64_t must_mask, int cap, int* n_out, uint64_t* off1, uint64_t* off2,
-    uint64_t* pmasks, double* mats8);
 int b200sv_finish(b200sv_t s); /* flush + wait for the device (QInterface::Finish) */
 /* mode 0: every gate is its own launch (reference-like); 1: fused multi-gate sweeps (default) */
 int b200sv_set_fusion(b200sv_t s, int mode);
@@ -264,17 +245,12 @@ int b200sv_apply_gates(b200sv_t s, int n_gates, const uint64_t* off1, const uint
  * pmasks[i]) in its single-target form.  `pytest -m "not gpu"` checks scheduler + encoder against the oracle with it. */
 int b200sv_emulate_fused(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2,
     const uint64_t* pmasks, const double* mats8, void* host_state);
-/* DIAGNOSTIC (host only): what one flush of this gate list would launch — fused sweeps, register passes, device ops */
+/* DIAGNOSTIC (host only): what one flush of this gate list would launch — fused sweeps, register passes, device ops
+ * (scripts/shard_sweep_count.py counts the sweeps of a sharded step with it) */
 int b200sv_plan_gates(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2,
     const uint64_t* pmasks, const double* mats8, int* n_sweeps, int* n_passes, int* n_ops);
-/* TEST HOOK (host only): b200sv_flush_carry on a host state (host_state may be NULL: plan only, for scripts/shard_sweep_count.py);
- * *n_sweeps = sweeps that ran */
-int b200sv_emulate_fused_carry(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2,
-    const uint64_t* pmasks, const double* mats8, void* host_state, int min_ops, uint64_t must_mask, int cap, int* n_out,
-    uint64_t* out_off1, uint64_t* out_off2, uint64_t* out_pmasks, double* out_mats8, int* n_sweeps, int n_virtual,
-    uint64_t rank);
-/* TEST HOOK (host only): the same with a pending b200sv_exchange_pull — src_states[r] are HOST arrays standing in for the
- * ranks' pages, out_state receives this rank's new page after the gates (first sweep reads through the pull mapping). */
+/* TEST HOOK (host only): b200sv_emulate_fused with a pending b200sv_exchange_pull — src_states[r] are HOST arrays standing in
+ * for the ranks' pages, out_state receives this rank's new page after the gates (first sweep reads through the pull mapping). */
 int b200sv_emulate_fused_pull(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2,
     const uint64_t* pmasks, const double* mats8, int k, const int* victim_bits, int rank, void* const* src_states,
     void* out_state);

@@ -100,18 +100,12 @@ SIGNATURES = {
     "b200sv_hash": [H, c_int, c_int, c_char_p],
     "b200sv_phase_flip_if_less": [H, c_uint64, c_int, c_int, c_int],
     "b200sv_flush": [H],
-    "b200sv_set_rank_bits": [H, c_int, c_uint64],
-    "b200sv_flush_carry": [H, c_int, c_uint64, c_int, POINTER(c_int), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64),
-                           POINTER(c_double)],
     "b200sv_finish": [H],
     "b200sv_set_fusion": [H, c_int],
     "b200sv_emulate_fused": [c_int, c_int, c_int, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_double),
                              c_void_p],
     "b200sv_plan_gates": [c_int, c_int, c_int, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_double),
                           POINTER(c_int), POINTER(c_int), POINTER(c_int)],
-    "b200sv_emulate_fused_carry": [c_int, c_int, c_int, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_double),
-                                   c_void_p, c_int, c_uint64, c_int, POINTER(c_int), POINTER(c_uint64), POINTER(c_uint64),
-                                   POINTER(c_uint64), POINTER(c_double), POINTER(c_int), c_int, c_uint64],
     "b200sv_emulate_fused_pull": [c_int, c_int, c_int, POINTER(c_uint64), POINTER(c_uint64), POINTER(c_uint64), POINTER(c_double),
                                   c_int, POINTER(c_int), c_int, POINTER(c_void_p), c_void_p],
     "b200sv_get_stats": [H, POINTER(Stats)],

@@ -1340,60 +1340,8 @@ static int launch_apply2x2(State* s, uint64_t off1, uint64_t off2, const double*
     double* normOutDev);
 
 // A queued gate back in its (offset1, offset2, powers) form on the generic kernel
-// Gates may name "virtual" qubits >= nq (b200sv_set_rank_bits), constant on this state: strip them.  Returns false when the gate
-// never fires here.  A diagonal gate whose own qubit is virtual leaves one diagonal entry d: a phase on its last real control
-// under the others, or a global scalar.
-static bool fold_virtual(const State* s, GateOp& g)
+static int run_gate_unfused(State* s, const GateOp& g)
 {
-    if (!s->nVirt) {
-        return true;
-    }
-    const uint64_t vm = ((1ULL << s->nVirt) - 1ULL) << s->nq;
-    if (g.cmask & vm) {
-        if ((g.cval & g.cmask & vm) != (s->virtVal & g.cmask & vm)) {
-            return false;
-        }
-        g.cmask &= ~vm;
-        g.cval &= ~vm;
-    }
-    if (g.target >= s->nq) {
-        const bool one = ((s->virtVal >> g.target) & 1ULL) != 0;
-        const double dx = one ? g.m[6] : g.m[0], dy = one ? g.m[7] : g.m[1];
-        if (dx == 1.0 && dy == 0.0) {
-            return false;
-        }
-        memset(g.m, 0, sizeof(g.m));
-        if (g.cmask) {
-            const int c = 63 - __builtin_clzll(g.cmask);
-            const bool want = ((g.cval >> c) & 1ULL) != 0;
-            g.cmask &= ~(1ULL << c);
-            g.cval &= ~(1ULL << c);
-            g.target = c;
-            if (want) {
-                g.m[0] = 1.0;
-                g.m[6] = dx;
-                g.m[7] = dy;
-            } else {
-                g.m[0] = dx;
-                g.m[1] = dy;
-                g.m[6] = 1.0;
-            }
-        } else {
-            g.target = 0;
-            g.m[0] = g.m[6] = dx;
-            g.m[1] = g.m[7] = dy;
-        }
-        g.kind = 1;
-    }
-    return true;
-}
-
-static int run_gate_unfused(State* s, const GateOp& gin)
-{
-    GateOp g = gin;
-    if (!fold_virtual(s, g)) {
-        return B200SV_OK;
-    }
     uint64_t pows[64];
     int nb = 0;
     const uint64_t pmask = g.cmask | (1ULL << g.target);
@@ -1840,58 +1788,6 @@ int b200sv_flush(b200sv_t s)
 {
     SV_ENTER_RO(s);
     return flush_queue(s);
-}
-
-static int copy_carry(const CarryReq& c, int cap, int* n_out, uint64_t* off1, uint64_t* off2, uint64_t* pmasks, double* mats8)
-{
-    const size_t n = c.off1.size();
-    if (n > (size_t)cap) {
-        set_error("flush_carry: internal error (more ops handed back than the caller's capacity)");
-        return B200SV_ESTATE;
-    }
-    for (size_t i = 0; i < n; ++i) {
-        off1[i] = c.off1[i];
-        off2[i] = c.off2[i];
-        pmasks[i] = c.pmask[i];
-    }
-    if (n) {
-        memcpy(mats8, c.m8.data(), n * 8 * sizeof(double));
-    }
-    *n_out = (int)n;
-    return B200SV_OK;
-}
-
-int b200sv_flush_carry(b200sv_t s, int min_ops, uint64_t must_mask, int cap, int* n_out, uint64_t* off1, uint64_t* off2,
-    uint64_t* pmasks, double* mats8)
-{
-    SV_ENTER_RO(s);
-    if (min_ops < 0 || cap < 0 || !n_out || (cap && (!off1 || !off2 || !pmasks || !mats8))) {
-        return einval("flush_carry: bad arguments");
-    }
-    *n_out = 0;
-    if (s->queue.empty() || !min_ops || !cap) {
-        return flush_queue(s);
-    }
-    std::vector<GateOp> saved;
-    const bool keep = s->queue.size() <= 8192;
-    if (keep) {
-        saved = s->queue;
-    }
-    CarryReq c;
-    c.minOps = (size_t)min_ops;
-    c.mustMask = must_mask;
-    c.cap = (size_t)cap;
-    const int rc = fused_flush(s, &c);
-    if (rc == B200SV_ESTATE && keep) { // planner gave up before anything was launched: gate by gate, nothing handed back
-        s->queue.clear();
-        SV_TRY(launch_pull_gather(s));
-        for (const GateOp& g : saved) {
-            SV_TRY(run_gate_unfused(s, g));
-        }
-        return B200SV_OK;
-    }
-    SV_TRY(rc);
-    return copy_carry(c, cap, n_out, off1, off2, pmasks, mats8);
 }
 
 int b200sv_finish(b200sv_t s)
@@ -2445,14 +2341,9 @@ int b200sv_apply_gates(b200sv_t s, int n_gates, const uint64_t* off1, const uint
     if (n_gates < 0 || (n_gates && (!off1 || !off2 || !pmasks || !mats8))) {
         return einval("apply_gates: null argument");
     }
-    const uint64_t dim = s->dim();
     for (int i = 0; i < n_gates; ++i) {
         const uint64_t diff = off1[i] ^ off2[i];
-        // controls (and the qubit of a DIAGONAL gate) may be virtual qubits when the state has them (b200sv_set_rank_bits)
-        const bool diagonal = mats8[8 * (size_t)i + 2] == 0 && mats8[8 * (size_t)i + 3] == 0 && mats8[8 * (size_t)i + 4] == 0 &&
-            mats8[8 * (size_t)i + 5] == 0;
-        if (!diff || (diff & (diff - 1U)) || (pmasks[i] >> (s->nq + s->nVirt)) || ((off1[i] | off2[i]) & ~pmasks[i]) ||
-            (diff >= dim && !diagonal)) {
+        if (!diff || (diff & (diff - 1U)) || (pmasks[i] >> s->nq) || ((off1[i] | off2[i]) & ~pmasks[i])) {
             return einval("apply_gates: every gate must be a single-target Apply2x2 form within the qubit bounds");
         }
     }
@@ -2474,18 +2365,6 @@ int b200sv_apply_gates(b200sv_t s, int n_gates, const uint64_t* off1, const uint
         SV_TRY(flush_queue(s));
         SV_TRY(run_gate_unfused(s, g));
     }
-    return B200SV_OK;
-}
-
-int b200sv_set_rank_bits(b200sv_t s, int k, uint64_t rank)
-{
-    SV_ENTER(s);
-    if (k < 0 || k > 16 || s->nq + k > 62 || (k < 64 && (rank >> k))) {
-        return einval("set_rank_bits: 0 <= k <= 16, rank < 2^k, nq + k <= 62");
-    }
-    SV_TRY(flush_queue(s)); // what is queued was submitted under the old rank bits
-    s->nVirt = k;
-    s->virtVal = rank << s->nq;
     return B200SV_OK;
 }
 
@@ -3679,35 +3558,6 @@ int b200sv_emulate_fused(int n_qubits, int precision, int n_gates, const uint64_
         make_gate_op(precision, off1[i], off2[i], pmasks[i], mats8 + 8 * (size_t)i, 1.0, q[(size_t)i]);
     }
     return fused_emulate(n_qubits, precision, q, host_state);
-}
-
-int b200sv_emulate_fused_carry(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2,
-    const uint64_t* pmasks, const double* mats8, void* host_state, int min_ops, uint64_t must_mask, int cap, int* n_out,
-    uint64_t* out_off1, uint64_t* out_off2, uint64_t* out_pmasks, double* out_mats8, int* n_sweeps, int n_virtual, uint64_t rank)
-{
-    if (n_gates < 0 || (n_gates && (!off1 || !off2 || !pmasks || !mats8)) || (precision != 32 && precision != 64) || n_qubits < 5 ||
-        n_qubits > 62 || (host_state && n_qubits > 30) || min_ops < 0 || cap < 0 || !n_out ||
-        (cap && (!out_off1 || !out_off2 || !out_pmasks || !out_mats8)) || n_virtual < 0 || n_virtual > 16 || n_qubits + n_virtual > 62 ||
-        (rank >> n_virtual)) {
-        return einval("emulate_fused_carry: bad arguments");
-    }
-    std::vector<GateOp> q((size_t)n_gates);
-    for (int i = 0; i < n_gates; ++i) {
-        const uint64_t diff = off1[i] ^ off2[i];
-        if (!diff || (diff & (diff - 1U)) || (pmasks[i] >> (n_qubits + n_virtual)) || ((off1[i] | off2[i]) & ~pmasks[i])) {
-            return einval("emulate_fused_carry: not a single-target gate");
-        }
-        make_gate_op(precision, off1[i], off2[i], pmasks[i], mats8 + 8 * (size_t)i, 1.0, q[(size_t)i]);
-    }
-    CarryReq c;
-    c.minOps = (size_t)min_ops;
-    c.mustMask = must_mask;
-    c.cap = (size_t)cap;
-    SV_TRY(fused_emulate(n_qubits, precision, q, host_state, nullptr, &c, n_virtual, rank << n_qubits));
-    if (n_sweeps) {
-        *n_sweeps = c.sweepsLaunched;
-    }
-    return copy_carry(c, cap, n_out, out_off1, out_off2, out_pmasks, out_mats8);
 }
 
 int b200sv_emulate_fused_pull(int n_qubits, int precision, int n_gates, const uint64_t* off1, const uint64_t* off2,

@@ -848,7 +848,6 @@ struct HostOp {
     uint64_t cmask; // predicate mask over qubits (controls; for OP_PHASE includes the phased qubit)
     uint64_t cval;
     double m[8];
-    int id; // position in the lowered list (set by plan_all when it needs to tell ops apart)
 };
 
 static inline uint64_t bitq(int q) { return 1ULL << q; }
@@ -1259,8 +1258,6 @@ struct TileCfg {
     int kA;   // tile amplitude bits actually used
     int H;    // capacity of high qubits
     int maxOps; // ops per sweep (bounded by the shared-memory program area)
-    // virtual qubits (>= n, State::nVirt): constant on this state; predicates on them are folded when the sweep is encoded
-    uint64_t virtMask = 0, virtVal = 0;
 };
 
 static TileCfg make_cfg(int n, int prec)
@@ -1795,17 +1792,7 @@ static size_t encode_sweep(const SweepPlan& sp, const TileCfg& cfg, std::vector<
             stage_reset();
         };
         dp.opBegin = (int)dops.size();
-        for (const HostOp& hopSym : pp.ops) {
-            // fold the predicate on virtual qubits (rank bits of a sharded register: constant here): the op either never fires on
-            // this state — nothing is emitted — or loses those bits
-            HostOp hop = hopSym;
-            if (hop.cmask & cfg.virtMask) {
-                if ((hop.cval & hop.cmask & cfg.virtMask) != (cfg.virtVal & hop.cmask & cfg.virtMask)) {
-                    continue;
-                }
-                hop.cmask &= ~cfg.virtMask;
-                hop.cval &= ~cfg.virtMask;
-            }
+        for (const HostOp& hop : pp.ops) {
             uint32_t lmask, lval;
             local_pred(hop, lmask, lval);
             const uint32_t lmr = lmask & regAmpMask, lvr = lval & regAmpMask;
@@ -2093,59 +2080,10 @@ struct Seg {
     int npass;
 };
 
-// a lowered op as a single-target gate (b200sv_apply_gates layout); a predicated phase takes its lowest predicate qubit as "target"
-static void export_op(const HostOp& h, CarryReq* c)
-{
-    double m[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    uint64_t o1 = 0, o2 = 0, pm = 0;
-    if (h.kind == OP_PHASE) {
-        if (!h.cmask) { // a global phase
-            m[0] = m[6] = h.m[0];
-            m[1] = m[7] = h.m[1];
-            o2 = pm = 1ULL;
-        } else {
-            const uint64_t tb = h.cmask & (~h.cmask + 1ULL);
-            o1 = h.cval & h.cmask & ~tb;
-            o2 = o1 | tb;
-            pm = h.cmask;
-            if (h.cval & tb) {
-                m[0] = 1.0;
-                m[6] = h.m[0];
-                m[7] = h.m[1];
-            } else {
-                m[0] = h.m[0];
-                m[1] = h.m[1];
-                m[6] = 1.0;
-            }
-        }
-    } else {
-        const uint64_t tb = bitq(h.tq);
-        o1 = h.cval & h.cmask;
-        o2 = o1 | tb;
-        pm = h.cmask | tb;
-        if (h.kind == OP_ROT) {
-            m[0] = h.m[0];
-            m[2] = -h.m[1];
-            m[4] = h.m[1];
-            m[6] = h.m[0];
-        } else {
-            memcpy(m, h.m, sizeof(m));
-        }
-    }
-    c->off1.push_back(o1);
-    c->off2.push_back(o2);
-    c->pmask.push_back(pm);
-    c->m8.insert(c->m8.end(), m, m + 8);
-}
-
-// Plans and encodes the sweeps of `pending` (consumed), nothing else.
-static int plan_list(std::vector<HostOp>& pending, const TileCfg& cfg, int prec, std::vector<unsigned char>& buf, std::vector<Seg>& segs,
-    std::vector<std::vector<HostOp>>* snaps)
+// Plans and encodes every sweep of a flush: `pending` is consumed.
+static int plan_list(std::vector<HostOp>& pending, const TileCfg& cfg, int prec, std::vector<unsigned char>& buf, std::vector<Seg>& segs)
 {
     while (!pending.empty()) {
-        if (snaps) {
-            snaps->push_back(pending);
-        }
         const size_t off = buf.size();
         size_t bytes = 0, scratch = 0, nops = 0;
         int npass = 0;
@@ -2154,131 +2092,6 @@ static int plan_list(std::vector<HostOp>& pending, const TileCfg& cfg, int prec,
         if (getenv("B200SV_FUSED_DEBUG")) {
             fprintf(stderr, "  program %zu B + scratch %zu B\n", bytes, scratch);
         }
-    }
-    return B200SV_OK;
-}
-
-// Plans and encodes every sweep of a flush.
-//
-// With `carry` the under-filled tail of the window is not executed.  Phase A decides WHAT is handed back, on the symbolic op list
-// (virtual-qubit predicates unfolded), so that every rank of a sharded register — same queue, deterministic planner —
-// takes the same decision: an exchange redistributes amplitudes between the ranks, an op executed before it on one rank and after
-// it on another would hit some amplitudes twice.  Candidate cuts: j = first sweep of a trailing run of sweeps that each hold fewer
-// than minOps ops.  Of what is left over at cut j (program order) the ops that MUST still run now are the non-diagonal ops on
-// mustMask qubits together with every earlier left-over op that does not commute with one of them (backward closure under the
-// scheduler's conflict rule: shared qubits must be used diagonally by both); they are planned on their own, everything else is
-// handed back (plus a trailing XMask as X gates; *xtail is cleared then).  The cut with the fewest sweeps in total wins (ties: the
-// latest cut = fewest ops handed back).  Phase B plans what is executed for THIS state: ops whose virtual-qubit predicate cannot
-// hold here are identities and are dropped, the others lose those bits.
-static int plan_all(std::vector<HostOp>& pending, const TileCfg& cfg, int prec, std::vector<unsigned char>& buf, std::vector<Seg>& segs,
-    CarryReq* carry, uint64_t* xtail)
-{
-    std::vector<HostOp> exec;
-    if (carry && carry->minOps && !pending.empty() && !(*xtail & carry->mustMask)) {
-        TileCfg sym = cfg;
-        sym.virtMask = sym.virtVal = 0;
-        for (size_t i = 0; i < pending.size(); ++i) {
-            pending[i].id = (int)i;
-        }
-        std::vector<HostOp> work = pending;
-        std::vector<std::vector<HostOp>> snaps;
-        std::vector<unsigned char> symBuf;
-        std::vector<Seg> symSegs;
-        SV_TRY(plan_list(work, sym, prec, symBuf, symSegs, &snaps));
-        size_t firstSmall = symSegs.size();
-        while (firstSmall > 0 && symSegs[firstSmall - 1].nops < carry->minOps) {
-            --firstSmall;
-        }
-        size_t bestTotal = symSegs.size();
-        bool found = false;
-        std::vector<HostOp> bestCarried;
-        for (size_t j = symSegs.size(); j-- > firstSmall;) {
-            const std::vector<HostOp>& left = snaps[j];
-            std::vector<char> must(left.size(), 0);
-            uint64_t mT = 0, mD = 0;
-            size_t nMust = 0;
-            for (size_t i = left.size(); i-- > 0;) {
-                const HostOp& h = left[i];
-                const uint64_t usesT = h.tq >= 0 ? bitq(h.tq) : 0;
-                const uint64_t usesD = h.cmask;
-                if ((usesT & carry->mustMask) || (usesT & (mT | mD)) || (usesD & mT)) {
-                    must[i] = 1;
-                    mT |= usesT;
-                    mD |= usesD;
-                    ++nMust;
-                }
-            }
-            if (left.size() - nMust + 64 > carry->cap) {
-                continue;
-            }
-            std::vector<HostOp> mustOps, carried;
-            for (size_t i = 0; i < left.size(); ++i) {
-                (must[i] ? mustOps : carried).push_back(left[i]);
-            }
-            std::vector<unsigned char> mbuf;
-            std::vector<Seg> msegs;
-            if (!mustOps.empty() && plan_list(mustOps, sym, prec, mbuf, msegs, nullptr) != B200SV_OK) {
-                continue;
-            }
-            const size_t total = j + msegs.size();
-            if (total < bestTotal) {
-                bestTotal = total;
-                found = true;
-                bestCarried.swap(carried);
-            }
-        }
-        if (found) {
-            std::vector<char> gone(pending.size(), 0);
-            for (const HostOp& h : bestCarried) {
-                gone[(size_t)h.id] = 1;
-                export_op(h, carry);
-            }
-            for (uint64_t m = *xtail; m; m &= m - 1ULL) { // the trailing XMask follows the carried ops
-                HostOp x;
-                memset(&x, 0, sizeof(x));
-                x.kind = OP_XSWAP;
-                x.tq = __builtin_ctzll(m);
-                x.m[2] = x.m[4] = 1.0;
-                export_op(x, carry);
-            }
-            *xtail = 0;
-            for (size_t i = 0; i < pending.size(); ++i) {
-                if (!gone[i]) {
-                    exec.push_back(pending[i]);
-                }
-            }
-        } else {
-            exec.swap(pending);
-        }
-    } else {
-        exec.swap(pending);
-    }
-    pending.clear();
-    if (cfg.virtMask) {
-        size_t w = 0;
-        bool changed = false;
-        for (size_t i = 0; i < exec.size(); ++i) {
-            HostOp h = exec[i];
-            if (h.cmask & cfg.virtMask) {
-                changed = true;
-                if ((h.cval & h.cmask & cfg.virtMask) != (cfg.virtVal & h.cmask & cfg.virtMask)) {
-                    continue; // cannot fire on this state: the identity
-                }
-                h.cmask &= ~cfg.virtMask;
-                h.cval &= ~cfg.virtMask;
-            }
-            exec[w++] = h;
-        }
-        exec.resize(w);
-        if (changed) {
-            // the peephole rules once more on what is left: the Hadamard pair around a controlled-X whose rank-bit control fails here is
-            // H . H now, a CZ that lost its rank-bit control is a Z to absorb, ...
-            *xtail ^= rewrite_ops(exec);
-        }
-    }
-    SV_TRY(plan_list(exec, cfg, prec, buf, segs, nullptr));
-    if (carry) {
-        carry->sweepsLaunched = (int)segs.size();
     }
     return B200SV_OK;
 }
@@ -2374,7 +2187,7 @@ static int launch_sweep(State* s, const unsigned char* dprog, uint32_t progBytes
                                 : launch_sweep_v<R, 0>(s, dprog, progBytes, scratchBytes, nTiles));
 }
 
-int fused_flush(State* s, CarryReq* carry)
+int fused_flush(State* s)
 {
     if (s->queue.empty()) {
         return s->pullPending ? launch_pull_gather(s) : B200SV_OK;
@@ -2384,15 +2197,13 @@ int fused_flush(State* s, CarryReq* carry)
         return B200SV_OK;
     }
     std::vector<HostOp> pending;
-    uint64_t xtail = lower_queue(s->queue, pending);
+    const uint64_t xtail = lower_queue(s->queue, pending);
     const size_t nGates = s->queue.size();
-    TileCfg cfg = make_cfg(s->nq, s->prec);
-    cfg.virtMask = s->nVirt ? (((1ULL << s->nVirt) - 1ULL) << s->nq) : 0ULL;
-    cfg.virtVal = s->virtVal;
+    const TileCfg cfg = make_cfg(s->nq, s->prec);
     // build every sweep of this flush (nothing is launched before the whole flush is planned: a planner failure leaves the state as it was)
     std::vector<unsigned char> buf;
     std::vector<Seg> segs;
-    SV_TRY(plan_all(pending, cfg, s->prec, buf, segs, carry, &xtail));
+    SV_TRY(plan_list(pending, cfg, s->prec, buf, segs));
     s->queue.clear();
     // A pending re-page rides on the first sweep when there is one; otherwise it is a plain gather.
     if (s->pullPending && segs.empty()) {
@@ -2745,20 +2556,14 @@ static void emulate_sweep(const unsigned char* prog, EmuC<R>* psi, int nq, const
     }
 }
 
-int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, void* host_state, const PullArgs* pull, CarryReq* carry,
-    int n_virtual, uint64_t virt_value)
+int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, void* host_state, const PullArgs* pull)
 {
     std::vector<HostOp> pending;
-    uint64_t xtail = lower_queue(q, pending);
-    TileCfg cfg = make_cfg(n_qubits, precision);
-    cfg.virtMask = n_virtual ? (((1ULL << n_virtual) - 1ULL) << n_qubits) : 0ULL;
-    cfg.virtVal = virt_value;
+    const uint64_t xtail = lower_queue(q, pending);
+    const TileCfg cfg = make_cfg(n_qubits, precision);
     std::vector<unsigned char> buf;
     std::vector<Seg> segs;
-    SV_TRY(plan_all(pending, cfg, precision, buf, segs, carry, &xtail));
-    if (!host_state) { // plan only (scripts/shard_sweep_count.py)
-        return B200SV_OK;
-    }
+    SV_TRY(plan_list(pending, cfg, precision, buf, segs));
     if (pull && segs.empty()) { // launch_pull_gather on the device
         const uint64_t dim = 1ULL << n_qubits;
         for (uint64_t i = 0; i < dim; ++i) {

@@ -109,11 +109,6 @@ struct State {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, evx = nullptr;
     int fusion = 1;
     std::vector<GateOp> queue;
-    // "virtual" qubits nq .. nq+nVirt-1 (b200sv_set_rank_bits): index bits this page does not hold — the rank index of a sharded
-    // register — with a constant value on this state.  Queued gates may use them as controls / phased qubits; the predicate is
-    // folded when a sweep is encoded (or a gate runs unfused), and ops handed back by b200sv_flush_carry keep them.
-    int nVirt = 0;
-    uint64_t virtVal = 0; // already shifted to bit nq
     bool pullPending = false; // see PullArgs
     PullArgs pull{};
     b200sv_stats stats{};
@@ -145,26 +140,13 @@ int cuda_fail(cudaError_t e, const char* what);
 
 int sm_count(int dev);
 
-// Request to leave the under-filled tail of a flush un-executed (b200sv_flush_carry): trailing sweeps that would hold fewer than
-// `minOps` lowered ops are not launched and their ops (everything not executed, in program order) are handed back as single-target
-// gates in the layout of b200sv_apply_gates — unless one of them is a non-diagonal op on a qubit of `mustMask`.
-struct CarryReq {
-    size_t minOps = 0;
-    uint64_t mustMask = 0;
-    size_t cap = 0; // at most this many ops may be handed back
-    std::vector<uint64_t> off1, off2, pmask;
-    std::vector<double> m8;
-    int sweepsLaunched = 0;
-};
-
 // fused.cu
-int fused_flush(State* s, CarryReq* carry = nullptr);
+int fused_flush(State* s);
 int launch_xmask(State* s, uint64_t mask); // the dedicated XMask permutation sweep (b200sv.cu); does not flush
 bool fused_accepts(const State* s, const GateOp& g);
 void fused_release(State* s);
 int launch_pull_gather(State* s); // the pending pull as a plain gather kernel (b200sv.cu); adopts the out page
-int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, void* host_state, const PullArgs* pull = nullptr,
-    CarryReq* carry = nullptr, int n_virtual = 0, uint64_t virt_value = 0);
+int fused_emulate(int n_qubits, int precision, const std::vector<GateOp>& q, void* host_state, const PullArgs* pull = nullptr);
 int fused_plan_gates(int n_qubits, int precision, const std::vector<GateOp>& q, int* n_sweeps, int* n_passes, int* n_ops);
 
 } // namespace b200sv

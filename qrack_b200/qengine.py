@@ -1449,11 +1449,6 @@ class QEngineHost:
 # CUDA backend over the C ABI
 # ================================================================================================================
 
-def unpack_gates(n, o1, o2, pm, m8):
-    """ctypes arrays in the b200sv_apply_gates layout -> [(off1, off2, pmask, [4 complex]), ...]"""
-    return [(o1[i], o2[i], pm[i], [complex(m8[8 * i + 2 * j], m8[8 * i + 2 * j + 1]) for j in range(4)]) for i in range(n)]
-
-
 class _CudaBackend:
     """Backend primitives over libb200sv.so (include/b200sv.h).  One b200sv handle."""
 
@@ -1506,22 +1501,6 @@ class _CudaBackend:
 
     def flush(self):
         self._ck(self.lib.b200sv_flush(self.h))
-
-    def set_rank_bits(self, k: int, rank: int):
-        """b200sv_set_rank_bits: the rank index of a sharded register as k constant virtual qubits above this page's own"""
-        self._ck(self.lib.b200sv_set_rank_bits(self.h, k, rank))
-
-    def flush_carry(self, min_ops: int, must_mask: int, cap: int = 4096):
-        """b200sv_flush_carry: launch the queued gates except the under-filled tail of the window; returns what was NOT executed as
-        [(off1, off2, pmask, [m00, m01, m10, m11]), ...] in program order (single-target Apply2x2 forms)"""
-        import ctypes
-        n = ctypes.c_int()
-        o1 = (ctypes.c_uint64 * cap)()
-        o2 = (ctypes.c_uint64 * cap)()
-        pm = (ctypes.c_uint64 * cap)()
-        m8 = (ctypes.c_double * (8 * cap))()
-        self._ck(self.lib.b200sv_flush_carry(self.h, min_ops, must_mask, cap, ctypes.byref(n), o1, o2, pm, m8))
-        return unpack_gates(n.value, o1, o2, pm, m8)
 
     def is_zero(self) -> bool:
         import ctypes

@@ -161,12 +161,6 @@ class P2PShardBuffers:
         self.live = 0
         self.pull = os.environ.get("B200SV_SHARD_PULL", "1") != "0"  # 0: the push kernel (b200sv_exchange_scatter), one pass per exchange
         self.engine = QEngineCUDA.over_buffer(self.pages[0], n_local, device_index, precision, random.Random(1))
-        # B200SV_SHARD_VIRT=1: the local engine knows the rank index as constant virtual qubits and gates go to it un-specialised
-        # (b200sv_set_rank_bits) — the precondition of the tail carry (B200SV_SHARD_CARRY).  Off by default: the
-        # carry removes nearly empty sweeps, but a saving in time has not been measured
-        self.virtual_rank_bits = os.environ.get("B200SV_SHARD_VIRT", "0") != "0"
-        if self.virtual_rank_bits:
-            self.engine.be.set_rank_bits(world.bit_length() - 1, rank)
         self.engine.be.set_stream(torch.cuda.current_stream(self.device).cuda_stream)
         self.zero_live()
         dist.barrier()
@@ -249,15 +243,6 @@ class _ShardedBackend:
         self.exchange_bytes = 0
         self.local_swaps = 0
         self._batch = []  # local single-target gates waiting for ONE b200sv_apply_gates call (SURVEY N4)
-        # Tail carry (b200sv_flush_carry): before an exchange the local engine launches its window EXCEPT trailing sweeps that would
-        # hold fewer than this many lowered ops; what was not executed comes back as gates, is relabelled and runs in the next window,
-        # where it merges into the dense first sweeps.  Every sweep streams the whole page whatever it holds, and a window cut by an
-        # exchange ends on one or two nearly empty ones.  0 = off.
-        self.carry_min_ops = int(os.environ.get("B200SV_SHARD_CARRY", "1000000"))
-        self.carried_ops = 0
-        self._virt = bool(getattr(shard, "virtual_rank_bits", False))
-        if not self._virt:
-            self.carry_min_ops = 0  # gates specialised for this rank here (rank-bit controls folded) must not cross an exchange
         # X gates are never executed: |psi_logical> = X^{xinv} |psi_stored>.  An X (XMask) toggles bits of `xinv`; every later
         # gate is conjugated (control polarities flip, a target's matrix becomes X m X), every index that goes to or comes
         # from the stored state is XORed.  QInterface::MACWrapper (include/qinterface.hpp:179-189) wraps each anti-controlled
@@ -588,13 +573,8 @@ class _ShardedBackend:
             self._submit_batch()
             if not deferred:
                 break
-            # the first deferred gate is blocked only by its rank-bit target: after the exchange it can run.  What the local engine
-            # handed back instead of executing (the under-filled tail of its window) was runnable before every deferred gate it does
-            # not commute with, so it opens the next window: straight into the local batch — its targets are still local (no victim
-            # among them).  It takes no part in the scan below: the handed-back ops differ from rank to rank (rank-bit controls drop
-            # gates per rank), and every scheduling decision (what runs, when to exchange, which victims) must be the same everywhere.
-            for g in self._exchange(deferred, 0):
-                self._run_local(g)
+            # the first deferred gate is blocked only by its rank-bit target: after the exchange it can run
+            self._exchange(deferred, 0)
             ops = deferred
 
     def _local_gate(self, ctrls, cperm, m, pt):
@@ -629,16 +609,6 @@ class _ShardedBackend:
 
     def _run_local(self, g: _Gate):
         nl = self.nl
-        if self._virt:
-            # the local engine holds the rank index as virtual qubits nl .. nl+k-1: the gate goes there as it is (controls on rank
-            # bits, diagonal gates on a rank-bit qubit included) and stays valid if it is handed back across an exchange
-            ctrls = [self.perm[c] for c in _bits(g.cmask)]
-            cperm = 0
-            for j, c in enumerate(_bits(g.cmask)):
-                if (g.cval >> c) & 1:
-                    cperm |= 1 << j
-            self._local_gate(ctrls, cperm, g.m, self.perm[g.t])
-            return
         ctrls, cperm = [], 0
         for c in _bits(g.cmask):
             pc = self.perm[c]
@@ -700,15 +670,6 @@ class _ShardedBackend:
             vbits = top
         else:
             vbits = sorted(self.perm[v] for v in victims)
-        carried: List[_Gate] = []
-        if self.carry_min_ops > 0 and self.world > 1 and not self.shard.needs_top:
-            fc = getattr(getattr(self.loc, "be", None), "flush_carry", None)
-            if fc is not None:
-                must = 0
-                for b in vbits:
-                    must |= 1 << b  # a non-diagonal op on a victim qubit has to run before the qubit leaves the page
-                carried = [self._gate_from_physical(x, inv) for x in fc(self.carry_min_ops, must)]
-                self.carried_ops += len(carried)
         if self.world > 1:
             self.exchange_bytes += self.shard.exchange(self.dist, self.world, self.rank, k, vbits)
         self.exchanges += 1
@@ -717,23 +678,6 @@ class _ShardedBackend:
             ql, qg = inv[pl], inv[pg]
             self.perm[ql], self.perm[qg] = pg, pl
             inv[pl], inv[pg] = qg, ql
-        return carried
-
-    @staticmethod
-    def _gate_from_physical(x, inv) -> _Gate:
-        """a single-target gate of the LOCAL engine (off1, off2, pmask, m over physical local positions) as a gate over logical qubits"""
-        off1, off2, pmask, m = x
-        diff = off1 ^ off2
-        pt = diff.bit_length() - 1
-        if off1 & diff:
-            m = [m[3], m[2], m[1], m[0]]
-        cmask = cval = 0
-        for c in _bits(pmask & ~diff):
-            q = inv[c]
-            cmask |= 1 << q
-            if (off1 >> c) & 1:
-                cval |= 1 << q
-        return _Gate(inv[pt], cmask, cval, list(m))
 
 
 class QEngineSharded(QEngineHost):

@@ -17,39 +17,26 @@ class _Be:
         self.owner = owner
         self.q = []
         self.lib = _abi.load()
-        self.virt = (0, 0)
-
-    def set_rank_bits(self, k, rank):
-        self.virt = (k, rank)
 
     def apply_gates(self, n, o1, o2, pm, m8):
         for i in range(n):
             self.q.append((o1[i], o2[i], pm[i], [m8[8 * i + j] for j in range(8)]))
+            if len(self.q) >= 4096:   # b200sv_apply_gates flushes a queue this long
+                self.flush()
 
-    def _plan(self, min_ops, must):
+    def flush(self):
         g, self.q = self.q, []
         n = len(g)
         if not n:
-            return []
-        cap = 4096
+            return
         o1 = (ctypes.c_uint64 * n)(*[x[0] for x in g])
         o2 = (ctypes.c_uint64 * n)(*[x[1] for x in g])
         pm = (ctypes.c_uint64 * n)(*[x[2] for x in g])
         m8 = (ctypes.c_double * (8 * n))(*[v for x in g for v in x[3]])
-        no, sw = ctypes.c_int(), ctypes.c_int()
-        bo1, bo2, bpm = (ctypes.c_uint64 * cap)(), (ctypes.c_uint64 * cap)(), (ctypes.c_uint64 * cap)()
-        bm8 = (ctypes.c_double * (8 * cap))()
-        _abi.check(self.lib, self.lib.b200sv_emulate_fused_carry(self.owner.n_local, 32, n, o1, o2, pm, m8, None, min_ops, must, cap,
-                                                                  ctypes.byref(no), bo1, bo2, bpm, bm8, ctypes.byref(sw), *self.virt))
-        self.owner.windows.append((n, sw.value, no.value))
-        from qrack_b200.qengine import unpack_gates
-        return unpack_gates(no.value, bo1, bo2, bpm, bm8)
-
-    def flush_carry(self, min_ops, must_mask, cap=4096):
-        return self._plan(min_ops, must_mask)
-
-    def flush(self):
-        self._plan(0, 0)
+        sweeps, passes, ops = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        _abi.check(self.lib, self.lib.b200sv_plan_gates(self.owner.n_local, 32, n, o1, o2, pm, m8, ctypes.byref(sweeps),
+                                                        ctypes.byref(passes), ctypes.byref(ops)))
+        self.owner.windows.append((n, sweeps.value))
 
 
 class _NullEngine:
@@ -58,7 +45,7 @@ class _NullEngine:
     n_local = 30
 
     def __init__(self):
-        self.windows = []   # (gates in, sweeps launched, ops handed back) per local flush
+        self.windows = []   # (gates in, sweeps launched) per local flush
         self.be = _Be(self)
 
     def Finish(self):
@@ -71,18 +58,16 @@ class _NullEngine:
 class _NullShard:
     min_victim_bit = 8
     needs_top = False
-    virtual_rank_bits = True
 
-    def __init__(self, world=1, rank=0):
+    def __init__(self):
         self.engine = _NullEngine()
-        self.engine.be.set_rank_bits(world.bit_length() - 1, rank)
         self.cuts = []
 
     def zero_live(self):
         pass
 
     def exchange(self, dist, world, rank, k, vbits):
-        self.engine.be.flush()   # what the real exchange does first (a no-op after flush_carry)
+        self.engine.be.flush()   # what the real exchange does first
         self.cuts.append(len(self.engine.windows))
         return 0
 
@@ -92,7 +77,7 @@ def windows(n_local, world, rank, text):
 
     class Eng(sharded.QEngineSharded):
         def _make_backend(self, n_qubits):
-            return sharded._ShardedBackend(n_qubits, 32, _NullShard(world, rank), None, world, rank)
+            return sharded._ShardedBackend(n_qubits, 32, _NullShard(), None, world, rank)
 
     def make(n, perm):
         return Eng(n, perm, random.Random(1), 1.0 + 0j, precision=32, world=world, rank=rank)
@@ -100,19 +85,18 @@ def windows(n_local, world, rank, text):
     q = regs[0]
     q.be.flush()
     q.be.shard.engine.be.flush()
-    return q.be.exchanges, q.be.shard.engine.windows, q.be.carried_ops
+    return q.be.exchanges, q.be.shard.engine.windows
 
 
 def report(name, n_local, world, text, ranks=(0,), verbose=True):
     out = []
     for rank in ranks:
-        ex, rows, carried = windows(n_local, world, rank, text)
-        gates, sweeps = sum(r[0] for r in rows), sum(r[1] for r in rows)
+        ex, rows = windows(n_local, world, rank, text)
+        sweeps = sum(r[1] for r in rows)
         out.append((ex, sweeps))
         if verbose:
-            print("%s world %d rank %d (carry < %s ops): %d exchanges, %d local flushes, %d sweeps; %d ops handed across exchanges" % (
-                name, world, rank, os.environ.get("B200SV_SHARD_CARRY", "24"), ex, len(rows), sweeps, carried))
-            print("   per flush (gates in / sweeps / ops handed back): " + " ".join("%d/%d/%d" % r for r in rows))
+            print("%s world %d rank %d: %d exchanges, %d local flushes, %d sweeps" % (name, world, rank, ex, len(rows), sweeps))
+            print("   per flush (gates in / sweeps): " + " ".join("%d/%d" % r for r in rows))
     return out
 
 

@@ -18,7 +18,7 @@ class _EmuBackend(_RestateBackend):
         self.queue = []
         self.flushes = 0
         for name in dir(_RestateBackend):
-            if name.startswith("_") or name in ("apply2x2", "fn", "finish", "xmask", "apply_gates", "flush_carry", "flush"):
+            if name.startswith("_") or name in ("apply2x2", "fn", "finish", "xmask", "apply_gates", "flush"):
                 continue
             attr = getattr(self, name)
             if callable(attr):
@@ -70,9 +70,6 @@ class _EmuBackend(_RestateBackend):
     def flush(self):
         if not self.queue:
             return
-        if getattr(self, "virt", (0, 0))[0]:
-            self.flush_carry(0, 0)   # (the plain hook has no rank bits; min_ops = 0 hands nothing back)
-            return
         q, self.queue = self.queue, []
         n, o1, o2, pm, mats = self._packed(q)
         self._alloc()
@@ -80,33 +77,10 @@ class _EmuBackend(_RestateBackend):
         _abi.check(self.abi_lib, rc)
         self.flushes += 1
 
-    def set_rank_bits(self, k, rank):
-        self.flush()
-        self.virt = (k, rank)
-
-    # ---- the two batch entry points of the CUDA backend the sharded engine uses (qengine._CudaBackend.apply_gates / flush_carry) ----
+    # ---- the batch entry point of the CUDA backend the sharded engine uses (qengine._CudaBackend.apply_gates) ----
     def apply_gates(self, n, off1, off2, pmasks, mats8):
         for i in range(n):
             self.queue.append((off1[i], off2[i], pmasks[i], [complex(mats8[8 * i + 2 * j], mats8[8 * i + 2 * j + 1]) for j in range(4)]))
-
-    def flush_carry(self, min_ops, must_mask, cap=4096):
-        """b200sv_flush_carry through the host interpreter: runs the window except its under-filled tail, returns the rest as gates"""
-        from qrack_b200.qengine import unpack_gates
-        if not self.queue:
-            return []
-        q, self.queue = self.queue, []
-        n, o1, o2, pm, mats = self._packed(q)
-        self._alloc()
-        no, sw = ctypes.c_int(), ctypes.c_int()
-        bo1, bo2, bpm = (ctypes.c_uint64 * cap)(), (ctypes.c_uint64 * cap)(), (ctypes.c_uint64 * cap)()
-        bm8 = (ctypes.c_double * (8 * cap))()
-        rc = self.abi_lib.b200sv_emulate_fused_carry(self.nq, self.precision, n, o1, o2, pm, mats, self.amps.ctypes.data_as(ctypes.c_void_p),
-                                                     min_ops, must_mask, cap, ctypes.byref(no), bo1, bo2, bpm, bm8, ctypes.byref(sw),
-                                                     *getattr(self, "virt", (0, 0)))
-        _abi.check(self.abi_lib, rc)
-        self.flushes += 1
-        self.carried = getattr(self, "carried", 0) + no.value
-        return unpack_gates(no.value, bo1, bo2, bpm, bm8)
 
 
 class QEngineEmu(QEngineHost):

@@ -1,6 +1,6 @@
 """Test-only shard for QEngineSharded over gloo with the semantics of P2PShardBuffers (the k rank bits are exchanged with ANY k
 local qubits) and a local engine whose gates go through the real fused planner + the host interpreter of its programs
-(emu_engine.QEngineEmu), including b200sv_flush_carry.  Lets `-m "not gpu"` tests run the sharded scheduler with tail carry on."""
+(emu_engine.QEngineEmu).  Lets `-m "not gpu"` tests run the sharded scheduler on the planner the CUDA engine runs."""
 import random
 
 import numpy as np
@@ -20,8 +20,6 @@ class EmuP2PShard:
         self.engine = QEngineEmu(n_local, 0, random.Random(1), 1.0 + 0j, False, False, precision=precision)
         self.device = "cpu"
         self.torch = torch
-        self.virtual_rank_bits = True
-        self.engine.be.set_rank_bits(world.bit_length() - 1, rank)
         self.zero_live()
 
     def zero_live(self):
@@ -34,7 +32,7 @@ class EmuP2PShard:
         return self.engine.be.amps.copy()
 
     def stats(self):
-        return {"carried": getattr(self.engine.be, "carried", 0), "flushes": self.engine.be.flushes}
+        return {"flushes": self.engine.be.flushes}
 
     def exchange(self, dist, world, rank, k, victim_bits):
         be = self.engine.be

@@ -181,14 +181,3 @@ def test_emulated_pull_exchange_equals_exchange_then_sweeps(prec, k, nl, n_gates
     assert lib.b200sv_emulate_fused_pull(nl, prec, 0, None, None, None, None, k, vbc, 0, src, ctypes.c_void_p(pages[0].ctypes.data)) \
         == _abi.B200SV_EINVAL
     assert lib.b200sv_emulate_fused_pull(nl, prec, 0, None, None, None, None, 4, vbc, 0, src, None) == _abi.B200SV_EINVAL
-
-
-@pytest.mark.parametrize("prec", [32, 64])
-def test_rank_bits_and_carry_on_the_host_interpreter(prec):
-    """b200sv_set_rank_bits + b200sv_flush_carry semantics (the same check body runs on the GPU in tests/test_zz_carry_gpu.py):
-    gates with controls / diagonal targets on virtual qubits, one flush vs carry + resubmission, for every rank value."""
-    from carry_checks import check_rank_bits_and_carry
-    handed = 0
-    for seed in range(3):
-        handed += check_rank_bits_and_carry(lambda n: QEngineEmu(n, 0, random.Random(1), 1.0 + 0j, False, False, precision=prec), prec, seed=seed)
-    assert handed > 0

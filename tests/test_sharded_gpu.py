@@ -27,8 +27,7 @@ def _worker(rank, world, port, text, prec, out_path, mode):
     import torch
     import torch.distributed as dist
     p2p = mode != "nccl"
-    os.environ["B200SV_SHARD_PULL"] = "1" if mode in ("pull", "pull_carry") else "0"
-    os.environ["B200SV_SHARD_VIRT"] = "1" if mode == "pull_carry" else "0"   # rank bits as virtual qubits + tail carry across exchanges
+    os.environ["B200SV_SHARD_PULL"] = "1" if mode == "pull" else "0"
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     torch.cuda.set_device(rank)
@@ -42,14 +41,12 @@ def _worker(rank, world, port, text, prec, out_path, mode):
         regs, results = qscript.run(text, make)
         st = regs[0].GetQuantumState()
         if rank == 0:
-            np.savez(out_path, state=st, exchanges=regs[0].be.exchanges, pull_sweeps=regs[0].be.shard.stats().get("pull_sweeps", 0),
-                     carried=regs[0].be.carried_ops)
+            np.savez(out_path, state=st, exchanges=regs[0].be.exchanges, pull_sweeps=regs[0].be.shard.stats().get("pull_sweeps", 0))
     finally:
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("mode", ["nccl", "push", "pull", "pull_carry"],
-                         ids=["nccl_all_to_all", "p2p_scatter_kernel", "p2p_pull_fused_into_sweep", "p2p_pull_and_tail_carry"])
+@pytest.mark.parametrize("mode", ["nccl", "push", "pull"], ids=["nccl_all_to_all", "p2p_scatter_kernel", "p2p_pull_fused_into_sweep"])
 @pytest.mark.parametrize("prec", [32, 64])
 def test_sharded_nccl_matches_oracle(prec, mode, tmp_path):
     world = 2 if _ngpu() < 4 else 4
@@ -68,11 +65,9 @@ def test_sharded_nccl_matches_oracle(prec, mode, tmp_path):
                 raise
     z = np.load(out)
     d = float(np.abs(z["state"].astype(np.complex128) - want[0].astype(np.complex128)).max())
-    assert d <= util.AMP_TOL[prec], (d, "ops carried across exchanges: %d" % int(z["carried"]))
+    assert d <= util.AMP_TOL[prec], d
     assert int(z["exchanges"]) >= 1
-    if mode != "pull_carry":
-        assert int(z["carried"]) == 0         # gates are specialised per rank on these routes: nothing may cross an exchange
-    if mode in ("pull", "pull_carry"):
+    if mode == "pull":
         assert int(z["pull_sweeps"]) >= 1     # the re-page really rode on a fused sweep (b200sv_exchange_pull)
     else:
         assert int(z["pull_sweeps"]) == 0
