@@ -122,8 +122,10 @@ public:
     real1_f ProbParity(const bitCapInt& mask) override;
     bool ForceMParity(const bitCapInt& mask, bool result, bool doForce = true) override;
     bitCapInt MAll() override;
-    using QInterface::HighestProbAll;
     bitCapInt HighestProbAll(); // device arg-max; the QInterface default asks ProbAll() for every permutation
+    // top n as a device radix select (the default asks ProbAll() for every permutation and keeps the best n by insertion);
+    // exact, without the default's early exit on its running sum.  n > maxQPower throws before anything is launched.
+    std::vector<bitCapInt> HighestProbAll(size_t n) override;
     real1_f FirstNonzeroPhase() override { return IsZeroAmplitude() ? ZERO_R1_F : QInterface::FirstNonzeroPhase(); }
     real1_f GetExpectation(bitLenInt valueStart, bitLenInt valueLength) override;
     // The QInterface defaults ask ProbAll(i) — one device round trip — for every basis state (qinterface.cpp:478-800); here a

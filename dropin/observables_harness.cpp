@@ -14,6 +14,7 @@
 //   ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}
 //   ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..
 //   GetReducedDensityMatrix <cs>          (prints the 2 4^n values of rho row-major, interleaved re / im)
+//   HighestProbAllN n                     (prints the n most probable basis states, QInterface::HighestProbAll(n))
 #include "qfactory.hpp"
 
 #include <cstdio>
@@ -77,6 +78,16 @@ int main(int argc, char** argv)
             int c, t;
             ts >> c >> t;
             q->CNOT((bitLenInt)c, (bitLenInt)t);
+            continue;
+        }
+        if (op == "HighestProbAllN") {
+            size_t n;
+            ts >> n;
+            printf("%s", op.c_str());
+            for (const bitCapInt& p : q->HighestProbAll(n)) {
+                printf(" %llu", (unsigned long long)(bitCapIntOcl)p);
+            }
+            printf("\n");
             continue;
         }
         int k;

@@ -726,6 +726,31 @@ bitCapInt QEngineCUDA::HighestProbAll()
     return bitCapInt((bitCapIntOcl)perm);
 }
 
+std::vector<bitCapInt> QEngineCUDA::HighestProbAll(size_t n)
+{
+    // the reference's edge rules (qinterface.cpp:962-973); the selection itself is exact, without the early exit on the
+    // running sum (INTEGRATION.md)
+    if (!n) {
+        return std::vector<bitCapInt>();
+    }
+    if (n == 1U) {
+        return std::vector<bitCapInt>{ HighestProbAll() };
+    }
+    if (bitCapInt((bitCapIntOcl)n) > maxQPower) {
+        throw std::invalid_argument("QInterface::HighestProbAll(n) requested more !");
+    }
+    if (doNormalize) {
+        NormalizeState();
+    }
+    std::vector<uint64_t> perms(n);
+    Check(b200sv_highest_probs(sv, (uint64_t)n, perms.data()));
+    std::vector<bitCapInt> out(n);
+    for (size_t t = 0U; t < n; ++t) {
+        out[t] = bitCapInt((bitCapIntOcl)perms[t]);
+    }
+    return out;
+}
+
 bitCapInt QEngineCUDA::MAll()
 {
     // QEngineCPU::MAll (state.cpp:2026-2050) with the cumulative search done on the device

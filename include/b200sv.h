@@ -161,6 +161,13 @@ int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, doubl
 int b200sv_reduced_density_matrix(b200sv_t s, int k, const int* qubits, double* out);
 /* index of the largest |psi|^2 (HighestProbAll :1995-2024) */
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm);
+/* The n most probable basis states (HighestProbAll(n), qinterface.cpp:962-1003): perms_out[0..n) sorted by
+ * P(i) = min(|psi_i|^2, 1) descending, then by index ascending, P computed in double (fp32: (double)re^2 + (double)im^2).
+ * Indices with P = 0 are never listed; when fewer than n have P > 0 the list ends with zeros.  Exact: the reference's early
+ * exit on its running sum is not reproduced.  Read-only; the zero state gives n zeros.  n = 0 does nothing.  B200SV_EINVAL
+ * when perms_out is NULL (n > 0) or n > 2^qubits; B200SV_ENOMEM when the device buffer (16 B per listed state, beyond 1 MiB)
+ * cannot be had. */
+int b200sv_highest_probs(b200sv_t s, uint64_t n, uint64_t* perms_out);
 /* smallest index i with |psi[i]|^2 > REAL1_EPSILON and cumulative cum = sum_{j<=i} |psi[j]|^2 > rnd or 1 - cum <= FP_NORM_EPSILON,
  * else the last index with |psi|^2 > REAL1_EPSILON, else 2^n - 1 (MAll :2026-2050) */
 int b200sv_sample(b200sv_t s, double rnd, uint64_t* perm);

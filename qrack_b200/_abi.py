@@ -77,6 +77,7 @@ SIGNATURES = {
     "b200sv_expectation_pauli": [H, c_uint64, c_uint64, POINTER(c_double)],
     "b200sv_reduced_density_matrix": [H, c_int, POINTER(c_int), POINTER(c_double)],
     "b200sv_highest_prob": [H, POINTER(c_uint64)],
+    "b200sv_highest_probs": [H, c_uint64, POINTER(c_uint64)],
     "b200sv_sample": [H, c_double, POINTER(c_uint64)],
     "b200sv_sample_many": [H, c_int, POINTER(c_double), POINTER(c_uint64)],
     "b200sv_compose": [H, H, c_int],

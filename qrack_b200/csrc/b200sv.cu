@@ -1420,6 +1420,7 @@ static int flush_queue(State* s)
 #include "alu_kernels.cuh"
 #include "observables.cuh"
 #include "rdm.cuh"
+#include "topn.cuh"
 
 using namespace b200sv;
 
@@ -3006,6 +3007,26 @@ int b200sv_highest_prob(b200sv_t s, uint64_t* perm)
     }
     *perm = bidx;
     return B200SV_OK;
+}
+
+int b200sv_highest_probs(b200sv_t s, uint64_t n, uint64_t* perms_out)
+{
+    SV_ENTER_RO(s);
+    if (!n) {
+        return B200SV_OK;
+    }
+    if (!perms_out) {
+        return einval("highest_probs: null out pointer");
+    }
+    if (n > s->dim()) {
+        return einval("highest_probs: n is larger than 2^qubits");
+    }
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        std::fill(perms_out, perms_out + n, 0U);
+        return B200SV_OK;
+    }
+    return launch_topn(s, n, perms_out);
 }
 
 int b200sv_sample(b200sv_t s, double rnd, uint64_t* perm)

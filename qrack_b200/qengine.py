@@ -1317,6 +1317,25 @@ class QEngineHost:
     def HighestProbAll(self) -> int:
         return self.be.highest_prob()
 
+    def HighestProbAllN(self, n: int) -> list:
+        """QInterface::HighestProbAll(size_t n) (src/qinterface/qinterface.cpp:962-1003; HighestProbAllN in the C API) as a
+        device radix select (b200sv_highest_probs) instead of 2^n ProbAll calls: the n indices of largest
+        P(i) = min(|psi_i|^2, 1), ties to the smaller index; P = 0 is never listed and the list ends with zeros when fewer than
+        n have P > 0.  The reference's edge rules: n = 0 gives [], n = 1 gives [HighestProbAll()], n > 2^qubits raises
+        ValueError; with doNormalize the state is normalised first, as the reference's first ProbAll does.  Unlike the
+        reference, which stops once its running sum leaves no room for a better state, the list is always exact (the two
+        differ only on an unnormalised state or at near-ties within the reference's float rounding)."""
+        n = int(n)
+        if not n:
+            return []
+        if n == 1:
+            return [self.HighestProbAll()]
+        if n > self.maxQPower:
+            raise ValueError("QInterface::HighestProbAll(n) requested more !")
+        if self.doNormalize:
+            self.NormalizeState()
+        return self.be.highest_probs(n)
+
     def ForceMParity(self, mask: int, result: bool, doForce: bool = True) -> bool:  # state.cpp:2052-2107
         if mask >= self.maxQPower:
             raise ValueError("ForceMParity mask out-of-bounds!")
@@ -1676,6 +1695,13 @@ class _CudaBackend:
         p = ctypes.c_uint64()
         self._ck(self.lib.b200sv_highest_prob(self.h, ctypes.byref(p)))
         return p.value
+
+    def highest_probs(self, n: int) -> list:
+        """the n most probable basis states, zero-filled past the last P > 0 (b200sv_highest_probs)"""
+        import ctypes
+        out = np.zeros(max(n, 1), dtype=np.uint64)
+        self._ck(self.lib.b200sv_highest_probs(self.h, n, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64))))
+        return [int(v) for v in out[:n]]
 
     def sample(self, rnd: float) -> int:
         import ctypes

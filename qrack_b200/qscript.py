@@ -36,6 +36,7 @@ Grammar (tokens are whitespace separated; ``<m8>`` = 8 reals = 4 complex row-maj
     ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}        (0 = I, 1 = X, 2 = Z, 3 = Y: include/pauli.hpp)
     ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..  (the U3 form of ExpVarUnitaryAll)
     GetReducedDensityMatrix <cs>      (the 2 4^n values of rho row-major, interleaved re / im; bit p of a row is qubit p of <cs>)
+    HighestProbAllN n                 (the n most probable basis states, most probable first: QInterface::HighestProbAll(n))
 """
 from __future__ import annotations
 
@@ -47,7 +48,7 @@ QUERY_OPS = {
     "Prob", "ProbAll", "ProbReg", "ProbMask", "ProbParity", "CProb", "ACProb", "GetAmplitude", "SumSqrDiff", "Norm",
     "ExpectationBitsAll", "VarianceBitsAll", "ExpectationBitsFactorized", "VarianceBitsFactorized",
     "ExpectationFloatsFactorized", "VarianceFloatsFactorized", "ExpectationPauliAll", "VariancePauliAll",
-    "ExpectationUnitaryAll", "VarianceUnitaryAll", "GetReducedDensityMatrix",
+    "ExpectationUnitaryAll", "VarianceUnitaryAll", "GetReducedDensityMatrix", "HighestProbAllN",
 }
 
 
@@ -236,6 +237,8 @@ def run(text: str, make_reg: Callable[[int, int], object]) -> Tuple[Dict[int, ob
                 for z in row:
                     vals += [float(z.real), float(z.imag)]
             results.append((op, tuple(vals)))
+        elif op == "HighestProbAllN":
+            results.append((op, tuple(float(p) for p in q.HighestProbAllN(int(t[1])))))
         else:
             raise ValueError("qscript: unknown op %r" % op)
     return regs, results
