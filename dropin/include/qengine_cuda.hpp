@@ -126,6 +126,10 @@ public:
     // top n as a device radix select (the default asks ProbAll() for every permutation and keeps the best n by insertion);
     // exact, without the default's early exit on its running sum.  n > maxQPower throws before anything is launched.
     std::vector<bitCapInt> HighestProbAll(size_t n) override;
+    // lossy checkpoints (the TurboQuant file of statevector_turboquant.hpp) encoded / decoded on the device for 1 <= p <= 6 and
+    // 1 <= b <= 16; other p or b go to the QInterface default.  An unreadable file zeroes the state, as QEngineCPU does.
+    void LossySaveStateVector(std::string f, int p = 6, int b = 4) override;
+    void LossyLoadStateVector(std::string f) override;
     real1_f FirstNonzeroPhase() override { return IsZeroAmplitude() ? ZERO_R1_F : QInterface::FirstNonzeroPhase(); }
     real1_f GetExpectation(bitLenInt valueStart, bitLenInt valueLength) override;
     // The QInterface defaults ask ProbAll(i) — one device round trip — for every basis state (qinterface.cpp:478-800); here a

@@ -15,6 +15,7 @@
 //   ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..
 //   GetReducedDensityMatrix <cs>          (prints the 2 4^n values of rho row-major, interleaved re / im)
 //   HighestProbAllN n                     (prints the n most probable basis states, QInterface::HighestProbAll(n))
+//   LossySave path p b | LossyLoad path  (LossySaveStateVector / LossyLoadStateVector)
 #include "qfactory.hpp"
 
 #include <cstdio>
@@ -78,6 +79,19 @@ int main(int argc, char** argv)
             int c, t;
             ts >> c >> t;
             q->CNOT((bitLenInt)c, (bitLenInt)t);
+            continue;
+        }
+        if (op == "LossySave") {
+            std::string f;
+            int p, b;
+            ts >> f >> p >> b;
+            q->LossySaveStateVector(f, p, b);
+            continue;
+        }
+        if (op == "LossyLoad") {
+            std::string f;
+            ts >> f;
+            q->LossyLoadStateVector(f);
             continue;
         }
         if (op == "HighestProbAllN") {

@@ -10,6 +10,8 @@
 
 #include <algorithm>
 #include <cstring>
+#include <fstream>
+#include <random>
 
 namespace Qrack {
 
@@ -749,6 +751,48 @@ std::vector<bitCapInt> QEngineCUDA::HighestProbAll(size_t n)
         out[t] = bitCapInt((bitCapIntOcl)perms[t]);
     }
     return out;
+}
+
+static bool LossyOnDevice(int p, int b) { return (p >= 1) && (p <= 6) && (b >= 1) && (b <= 16); }
+
+void QEngineCUDA::LossySaveStateVector(std::string f, int p, int b)
+{
+    // QEngineCUDA (cuda.cu:3017-3035) / QEngineCPU (state.cpp:256-272): normalise first, p = 0 means p = qubitCount
+    if (!p) {
+        p = (int)qubitCount;
+    }
+    if (!LossyOnDevice(p, b)) {
+        return QInterface::LossySaveStateVector(f, p, b);
+    }
+    if (doNormalize) {
+        NormalizeState();
+    }
+    std::random_device rd;
+    const uint64_t seed = ((uint64_t)rd() << 32U) | (uint64_t)rd();
+    Check(b200sv_lossy_save(sv, f.c_str(), p, b, seed));
+}
+
+void QEngineCUDA::LossyLoadStateVector(std::string f)
+{
+    if (doNormalize) {
+        NormalizeState();
+    }
+    if (!std::ifstream(f).good()) {
+        // QEngineCPU (state.cpp:284-289) drops its state; the reference's CUDA engine would read garbage
+        return ZeroAmplitudes();
+    }
+    int nq = 0, p = 0, b = 0;
+    Check(b200sv_lossy_probe(f.c_str(), (int)(8U * sizeof(real1)), &nq, &p, &b));
+    if (!LossyOnDevice(p, b)) {
+        return QInterface::LossyLoadStateVector(f);
+    }
+    if ((bitLenInt)nq > qubitCount) {
+        Allocate(qubitCount, (bitLenInt)nq - qubitCount);
+    } else if ((bitLenInt)nq < qubitCount) {
+        Dispose(0U, qubitCount - (bitLenInt)nq);
+    }
+    Check(b200sv_lossy_load(sv, f.c_str()));
+    runningNorm = REAL1_DEFAULT_ARG;
 }
 
 bitCapInt QEngineCUDA::MAll()

@@ -168,6 +168,24 @@ int b200sv_highest_prob(b200sv_t s, uint64_t* perm);
  * when perms_out is NULL (n > 0) or n > 2^qubits; B200SV_ENOMEM when the device buffer (16 B per listed state, beyond 1 MiB)
  * cannot be had. */
 int b200sv_highest_probs(b200sv_t s, uint64_t n, uint64_t* perms_out);
+/* LossySaveStateVector (reference include/statevector_turboquant.hpp; QEngineCUDA cuda.cu:3017-3035): writes the TurboQuant
+ * file of the current state to `path`, block power p (1..6), `bits` per coordinate (1..16), every block rotated by the
+ * rotation of `seed`.  Bit-exact with the reference codec in plain sequential IEEE arithmetic.  Read-only: queued gates are
+ * flushed, the state and the memoised marginals are kept.  The zero state is encoded without a launch.  B200SV_EINVAL for a
+ * NULL path, p or bits out of range, or a file that cannot be written. */
+int b200sv_lossy_save(b200sv_t s, const char* path, int p, int bits, uint64_t seed);
+/* header + record geometry of a file for a state of `precision` (32 / 64): its qubit count (the adapter resizes before
+ * loading), block power and bits.  B200SV_EINVAL when the file cannot be opened, its capacity is not a power of two,
+ * num_blocks does not match, or the first record's D or NWORDS does not (a file of the other precision). */
+int b200sv_lossy_probe(const char* path, int precision, int* n_qubits, int* p, int* bits);
+/* LossyLoadStateVector: decodes the file into s, whose qubit count must equal the file's.  One rotation is built per distinct
+ * seed.  B200SV_EINVAL (state untouched) for a file that cannot be opened, a qubit count that differs, p outside 1..6, a
+ * block whose D is not BLOCK, BITS differing between blocks or outside 1..16, NWORDS not (2 D BITS + 63) / 64, a capacity
+ * that is not a power of two, or a length that does not match the state's precision; a malformed record found after the
+ * first chunk of 64 MiB of staging has been decoded leaves the zero state. */
+int b200sv_lossy_load(b200sv_t s, const char* path);
+/* TEST HOOK (host only): the dim x dim column-major rotation of `seed` in the given precision (32: float, 64: double) */
+int b200sv_lossy_rotation(int dim, int precision, uint64_t seed, void* out);
 /* smallest index i with |psi[i]|^2 > REAL1_EPSILON and cumulative cum = sum_{j<=i} |psi[j]|^2 > rnd or 1 - cum <= FP_NORM_EPSILON,
  * else the last index with |psi|^2 > REAL1_EPSILON, else 2^n - 1 (MAll :2026-2050) */
 int b200sv_sample(b200sv_t s, double rnd, uint64_t* perm);

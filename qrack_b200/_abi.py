@@ -11,7 +11,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200SV_LIB") or os.path.join(_HERE, "libb200sv.so")
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["b200sv.cu", "fused.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+# -ffp-contract=off: the host half of the lossy codec (the rotation) must keep every multiply and add separate
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC,-ffp-contract=off",
               "-shared", "-cudart", "static"]
 
 B200SV_OK, B200SV_EINVAL, B200SV_ENOMEM, B200SV_ECUDA, B200SV_ESTATE = 0, -1, -2, -3, -4
@@ -78,6 +79,10 @@ SIGNATURES = {
     "b200sv_reduced_density_matrix": [H, c_int, POINTER(c_int), POINTER(c_double)],
     "b200sv_highest_prob": [H, POINTER(c_uint64)],
     "b200sv_highest_probs": [H, c_uint64, POINTER(c_uint64)],
+    "b200sv_lossy_save": [H, c_char_p, c_int, c_int, c_uint64],
+    "b200sv_lossy_probe": [c_char_p, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)],
+    "b200sv_lossy_load": [H, c_char_p],
+    "b200sv_lossy_rotation": [c_int, c_int, c_uint64, c_void_p],
     "b200sv_sample": [H, c_double, POINTER(c_uint64)],
     "b200sv_sample_many": [H, c_int, POINTER(c_double), POINTER(c_uint64)],
     "b200sv_compose": [H, H, c_int],
@@ -173,3 +178,18 @@ def create(lib, device: int, n_qubits: int, precision: int, external_ptr: int = 
     else:
         check(lib, lib.b200sv_create(device, n_qubits, precision, ctypes.byref(h)))
     return h
+
+
+def lossy_probe(lib, path: str, precision: int):
+    """(qubits, p, bits) of a TurboQuant file read as `precision` (b200sv_lossy_probe)"""
+    n, p, b = c_int(), c_int(), c_int()
+    check(lib, lib.b200sv_lossy_probe(os.fsencode(path), precision, ctypes.byref(n), ctypes.byref(p), ctypes.byref(b)))
+    return n.value, p.value, b.value
+
+
+def lossy_rotation(lib, dim: int, precision: int, seed: int):
+    """the dim x dim rotation of `seed`, as stored (column-major, flattened), in float32 / float64 (b200sv_lossy_rotation)"""
+    import numpy as np
+    out = np.empty(dim * dim, dtype=np.float32 if precision == 32 else np.float64)
+    check(lib, lib.b200sv_lossy_rotation(dim, precision, seed, out.ctypes.data_as(c_void_p)))
+    return out

@@ -1421,6 +1421,7 @@ static int flush_queue(State* s)
 #include "observables.cuh"
 #include "rdm.cuh"
 #include "topn.cuh"
+#include "lossy.cuh"
 
 using namespace b200sv;
 
@@ -3027,6 +3028,57 @@ int b200sv_highest_probs(b200sv_t s, uint64_t n, uint64_t* perms_out)
         return B200SV_OK;
     }
     return launch_topn(s, n, perms_out);
+}
+
+int b200sv_lossy_save(b200sv_t s, const char* path, int p, int bits, uint64_t seed)
+{
+    SV_ENTER_RO(s);
+    if (!path) {
+        return einval("lossy_save: null path");
+    }
+    if (p < 1 || p > 6) {
+        return einval("lossy_save: block power p outside the device range 1..6");
+    }
+    if (bits < 1 || bits > 16) {
+        return einval("lossy_save: bits outside 1..16");
+    }
+    SV_TRY(flush_queue(s));
+    return (s->prec == 32) ? lossy_save_t<float>(s, path, p, bits, seed) : lossy_save_t<double>(s, path, p, bits, seed);
+}
+
+int b200sv_lossy_probe(const char* path, int precision, int* n_qubits, int* p, int* bits)
+{
+    if (!path || !n_qubits || !p || !bits) {
+        return einval("lossy_probe: null argument");
+    }
+    if (precision != 32 && precision != 64) {
+        return einval("lossy_probe: precision must be 32 or 64");
+    }
+    return lossy_probe_impl(path, precision, n_qubits, p, bits);
+}
+
+int b200sv_lossy_load(b200sv_t s, const char* path)
+{
+    SV_ENTER(s);
+    if (!path) {
+        return einval("lossy_load: null path");
+    }
+    return (s->prec == 32) ? lossy_load_t<float>(s, path) : lossy_load_t<double>(s, path);
+}
+
+int b200sv_lossy_rotation(int dim, int precision, uint64_t seed, void* out)
+{
+    if (!out || dim < 1 || dim > 4096) {
+        return einval("lossy_rotation: null output or dim outside 1..4096");
+    }
+    if (precision == 32) {
+        lossy_rotation_host<float>(dim, seed, (float*)out);
+    } else if (precision == 64) {
+        lossy_rotation_host<double>(dim, seed, (double*)out);
+    } else {
+        return einval("lossy_rotation: precision must be 32 or 64");
+    }
+    return B200SV_OK;
 }
 
 int b200sv_sample(b200sv_t s, double rnd, uint64_t* perm)

@@ -18,6 +18,7 @@ from __future__ import annotations
 
 import cmath
 import math
+import os
 import random
 from typing import List, Optional, Sequence
 
@@ -1336,6 +1337,48 @@ class QEngineHost:
             self.NormalizeState()
         return self.be.highest_probs(n)
 
+    # lossy checkpoints: the TurboQuant file of include/statevector_turboquant.hpp, encoded and decoded on the device
+    LOSSY_P_RANGE, LOSSY_B_RANGE = (1, 6), (1, 16)
+
+    def LossySaveStateVector(self, f: str, p: int = 6, b: int = 4):
+        """QInterface::LossySaveStateVector (QEngineCUDA cuda.cu:3017-3035): write the TurboQuant file of the state, block
+        power p (0 = qubitCount), b bits per coordinate, rotation seed (rd() << 32) | rd() from the OS entropy source.  There
+        is no host codec here, so p outside 1..6 or b outside 1..16 raises ValueError.  Normalises first with doNormalize."""
+        p = int(p) or self.qubitCount
+        b = int(b)
+        if not (self.LOSSY_P_RANGE[0] <= p <= self.LOSSY_P_RANGE[1] and self.LOSSY_B_RANGE[0] <= b <= self.LOSSY_B_RANGE[1]):
+            raise ValueError("LossySaveStateVector: the device codec covers 1 <= p <= 6 and 1 <= b <= 16 (got p = %d, b = %d)"
+                             % (p, b))
+        save = self.be.lossy_save
+        if self.doNormalize:
+            self.NormalizeState()
+        rd = random.SystemRandom()
+        save(f, p, b, (rd.getrandbits(32) << 32) | rd.getrandbits(32))
+
+    def LossyLoadStateVector(self, f: str):
+        """QInterface::LossyLoadStateVector: a file that cannot be opened zeroes the state (QEngineCPU state.cpp:284-289);
+        otherwise the register is resized to the file's qubit count (Allocate / Dispose(0, ..), as the reference does) and the
+        file is decoded on the device.  The running norm becomes unknown, as after SetQuantumState."""
+        load = self.be.lossy_load  # a backend without the primitive refuses before anything changes
+        if self.doNormalize:
+            self.NormalizeState()
+        try:
+            open(f, "rb").close()
+        except OSError:
+            self.ZeroAmplitudes()
+            return
+        from . import _abi
+        nq, p, b = _abi.lossy_probe(_abi.load(), f, self.precision)
+        if not (self.LOSSY_P_RANGE[0] <= p <= self.LOSSY_P_RANGE[1] and self.LOSSY_B_RANGE[0] <= b <= self.LOSSY_B_RANGE[1]):
+            raise ValueError("LossyLoadStateVector: the device codec covers 1 <= p <= 6 and 1 <= b <= 16 (file: p = %d, b = %d)"
+                             % (p, b))
+        if nq > self.qubitCount:
+            self.Allocate(self.qubitCount, nq - self.qubitCount)
+        elif nq < self.qubitCount:
+            self.Dispose(0, self.qubitCount - nq)
+        load(f)
+        self.runningNorm = REAL1_DEFAULT_ARG
+
     def ForceMParity(self, mask: int, result: bool, doForce: bool = True) -> bool:  # state.cpp:2052-2107
         if mask >= self.maxQPower:
             raise ValueError("ForceMParity mask out-of-bounds!")
@@ -1702,6 +1745,14 @@ class _CudaBackend:
         out = np.zeros(max(n, 1), dtype=np.uint64)
         self._ck(self.lib.b200sv_highest_probs(self.h, n, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64))))
         return [int(v) for v in out[:n]]
+
+    def lossy_save(self, path: str, p: int, bits: int, seed: int):
+        """the TurboQuant file of the state (b200sv_lossy_save)"""
+        self._ck(self.lib.b200sv_lossy_save(self.h, os.fsencode(path), p, bits, seed))
+
+    def lossy_load(self, path: str):
+        """decode a TurboQuant file into the state (b200sv_lossy_load)"""
+        self._ck(self.lib.b200sv_lossy_load(self.h, os.fsencode(path)))
 
     def sample(self, rnd: float) -> int:
         import ctypes

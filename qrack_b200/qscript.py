@@ -26,6 +26,8 @@ Grammar (tokens are whitespace separated; ``<m8>`` = 8 reals = 4 complex row-maj
     INC|DEC value start length
     SetPermutation perm   ForceM q result   ForceMReg start length result
     NormalizeState   UpdateRunningNorm
+    LossySave path p b   LossyLoad path            (LossySaveStateVector / LossyLoadStateVector; path has no spaces;
+                                                   replayed by the Python engines and dropin/observables_harness.cpp)
     Compose SRC [start]   Decompose start length DST   Dispose start length [perm]   Allocate start length
   queries (each appends one line to the results):
     Prob q   ProbAll perm   ProbReg start length perm   ProbMask mask perm   ProbParity mask
@@ -184,6 +186,10 @@ def run(text: str, make_reg: Callable[[int, int], object]) -> Tuple[Dict[int, ob
             q.NormalizeState()
         elif op == "UpdateRunningNorm":
             q.UpdateRunningNorm()
+        elif op == "LossySave":
+            q.LossySaveStateVector(t[1], int(t[2]), int(t[3]))
+        elif op == "LossyLoad":
+            q.LossyLoadStateVector(t[1])
         elif op == "Compose":
             if len(t) > 2:
                 q.Compose(regs[int(t[1])], int(t[2]))
