@@ -381,9 +381,7 @@ static int lossy_launch_t(State* s, bool encode, uint64_t blk0, uint64_t nblk, c
         k_lossy_decode<real, D2><<<grid, LOSSY_THREADS, smem, s->stream>>>((real*)s->amps, nreal, blk0, nblk, blist, M, bits,
                                                                            nwords, scales, words);
     }
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
-    return B200SV_OK;
+    return launched(s);
 }
 
 template <typename real>
@@ -447,33 +445,23 @@ struct LqFile {
 
 // device and pinned staging of one chunk, freed on every exit path
 template <typename real> struct LqStage {
-    real* d_scales = nullptr;
-    unsigned long long* d_words = nullptr;
-    real* d_mat = nullptr;
-    unsigned* d_list = nullptr;
-    real* h_scales = nullptr;
-    unsigned long long* h_words = nullptr;
-    unsigned* h_list = nullptr;
-    ~LqStage()
-    {
-        cudaFree(d_scales);
-        cudaFree(d_words);
-        cudaFree(d_mat);
-        cudaFree(d_list);
-        cudaFreeHost(h_scales);
-        cudaFreeHost(h_words);
-        cudaFreeHost(h_list);
-    }
+    DevBuf<real> d_scales;
+    DevBuf<unsigned long long> d_words;
+    DevBuf<real> d_mat;
+    DevBuf<unsigned> d_list;
+    PinnedBuf<real> h_scales;
+    PinnedBuf<unsigned long long> h_words;
+    PinnedBuf<unsigned> h_list;
     int alloc(size_t cb, int nwords, int d, bool lists)
     {
-        SV_CUDA(cudaMalloc(&d_scales, cb * sizeof(real)));
-        SV_CUDA(cudaMalloc(&d_words, cb * nwords * 8));
-        SV_CUDA(cudaMalloc(&d_mat, (size_t)d * d * sizeof(real)));
-        SV_CUDA(cudaMallocHost(&h_scales, cb * sizeof(real)));
-        SV_CUDA(cudaMallocHost(&h_words, cb * nwords * 8));
+        SV_CUDA(cudaMalloc(&d_scales.p, cb * sizeof(real)));
+        SV_CUDA(cudaMalloc(&d_words.p, cb * nwords * 8));
+        SV_CUDA(cudaMalloc(&d_mat.p, (size_t)d * d * sizeof(real)));
+        SV_CUDA(cudaMallocHost(&h_scales.p, cb * sizeof(real)));
+        SV_CUDA(cudaMallocHost(&h_words.p, cb * nwords * 8));
         if (lists) {
-            SV_CUDA(cudaMalloc(&d_list, cb * sizeof(unsigned)));
-            SV_CUDA(cudaMallocHost(&h_list, cb * sizeof(unsigned)));
+            SV_CUDA(cudaMalloc(&d_list.p, cb * sizeof(unsigned)));
+            SV_CUDA(cudaMallocHost(&h_list.p, cb * sizeof(unsigned)));
         }
         return B200SV_OK;
     }
@@ -815,7 +803,7 @@ template <typename real> static int lossy_load_t(State* s, const char* path)
     if (rc != B200SV_OK && touched) {
         // a record past the first chunk was malformed after part of the state was overwritten: leave the zero state
         if (s->external) {
-            cudaMemsetAsync(s->amps, 0, (size_t)s->dim() * s->amp_bytes(), s->stream);
+            SV_CUDA(cudaMemsetAsync(s->amps, 0, (size_t)s->dim() * s->amp_bytes(), s->stream));
         } else {
             free_amps(s);
         }

@@ -205,21 +205,16 @@ static int launch_moments(State* s, bool prod, int k, const int* bits, const uin
     const unsigned grid = stream_grid(s->dev, (s->prec == 32 && n >= 2) ? (n >> 1) : n, 256);
     const size_t shm = ((size_t)mt.n << 8) * 8U;
     const void* tabs = s->d_scratch + 4;
-    if (s->prec == 32) {
+    SV_TRY(with_prec(s, [&](auto r) {
+        using R = decltype(r);
+        const typename Cx<R>::type* psi = (const typename Cx<R>::type*)s->amps;
         if (prod) {
-            k_moments<float, true><<<grid, 256, shm, s->stream>>>((const float2*)s->amps, n, tabs, mt, offset, center, s->d_scratch);
+            k_moments<R, true><<<grid, 256, shm, s->stream>>>(psi, n, tabs, mt, offset, center, s->d_scratch);
         } else {
-            k_moments<float, false><<<grid, 256, shm, s->stream>>>((const float2*)s->amps, n, tabs, mt, offset, center, s->d_scratch);
+            k_moments<R, false><<<grid, 256, shm, s->stream>>>(psi, n, tabs, mt, offset, center, s->d_scratch);
         }
-    } else {
-        if (prod) {
-            k_moments<double, true><<<grid, 256, shm, s->stream>>>((const double2*)s->amps, n, tabs, mt, offset, center, s->d_scratch);
-        } else {
-            k_moments<double, false><<<grid, 256, shm, s->stream>>>((const double2*)s->amps, n, tabs, mt, offset, center, s->d_scratch);
-        }
-    }
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
+        return launched(s);
+    }));
     SV_TRY(read_scratch(s, 3));
     memcpy(out, s->h_scratch, 3 * sizeof(double));
     return B200SV_OK;
@@ -237,16 +232,13 @@ static int launch_pauli(State* s, uint64_t x, uint64_t z, double* out)
         items = units >> 1;
         topLow = (1ULL << (63 - __builtin_clzll(xu))) - 1U;
     }
-    SV_CUDA(cudaMemsetAsync(s->d_scratch, 0, 3 * sizeof(double), s->stream));
     const unsigned grid = stream_grid(s->dev, items, 256);
-    if (s->prec == 32) {
-        k_pauli<float><<<grid, 256, 0, s->stream>>>((const float2*)s->amps, n, items, x, z, topLow, s->d_scratch);
-    } else {
-        k_pauli<double><<<grid, 256, 0, s->stream>>>((const double2*)s->amps, n, items, x, z, topLow, s->d_scratch);
-    }
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
-    SV_TRY(read_scratch(s, 3));
+    SV_TRY(with_prec(s, [&](auto r) {
+        using R = decltype(r);
+        return scratch_reduce(s, 3, [&] {
+            k_pauli<R><<<grid, 256, 0, s->stream>>>((const typename Cx<R>::type*)s->amps, n, items, x, z, topLow, s->d_scratch);
+        });
+    }));
     const double re = s->h_scratch[1], im = s->h_scratch[2];
     out[0] = s->h_scratch[0];
     if (!x) {

@@ -235,54 +235,35 @@ static int launch_rdm(State* s, int k, const int* qubits, double* out)
     a.cols = 1ULL << (s->nq - k);
     a.slabs = (a.cols + S - 1) / S;
     a.rowsFast = (k > 0 && sorted[0] == 0) ? 1 : 0;
-    typedef void (*Kern)(const void*, RdmArgs, double*);
-    const bool f32 = s->prec == 32;
-    const Kern kern = (D >= 4) ? (f32 ? k_rdm<float, 4> : k_rdm<double, 4>)
-        : (D == 2)             ? (f32 ? k_rdm<float, 2> : k_rdm<double, 2>)
-                               : (f32 ? k_rdm<float, 1> : k_rdm<double, 1>);
     const size_t shm = 2 * RDM_SLAB * sizeof(double2) + 2 * D * sizeof(uint64_t);
     const uint64_t tiles = (uint64_t)a.nt * (a.nt + 1) / 2;
     const int sms = sm_count(s->dev);
-    // one tile: the environment split over every CTA that fits on the device at once, so the state is read once at full
-    // occupancy; several tiles: at least 2 x SMs CTAs in all
-    int perSm = 2;
-    SV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kern, RDM_THREADS, shm));
-    const uint64_t want = (tiles == 1) ? (uint64_t)sms * std::max(perSm, 1) : (2U * sms + tiles - 1) / tiles;
-    const unsigned splits = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want, a.slabs));
-
     const size_t dim = (size_t)1 << k;
     const size_t words = 2 * dim * dim;
     // the device sum: the state's scratch up to 1 MiB (k <= 8), else a buffer for this call only
-    const bool inScratch = words * sizeof(double) <= ((size_t)1 << 20);
-    double* dOut = nullptr;
-    if (inScratch) {
-        SV_TRY(ensure_scratch(s, words));
-        dOut = s->d_scratch;
-    } else {
-        SV_CUDA(cudaMalloc(&dOut, words * sizeof(double)));
-    }
+    DevBuf<> own;
+    void* dOut = nullptr;
+    SV_TRY(scratch_or_own(s, 0, words * sizeof(double), own, &dOut));
     std::vector<double> host;
-    int rc = B200SV_OK;
-    auto run = [&]() -> int {
-        SV_CUDA(cudaMemsetAsync(dOut, 0, words * sizeof(double), s->stream));
-        kern<<<dim3((unsigned)tiles, splits), RDM_THREADS, shm, s->stream>>>(s->amps, a, dOut);
-        SV_CUDA(cudaGetLastError());
-        s->stats.kernel_launches++;
-        if (inScratch) {
-            SV_CUDA(cudaMemcpyAsync(s->h_scratch, dOut, words * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
-        } else {
-            host.resize(words);
-            SV_CUDA(cudaMemcpyAsync(host.data(), dOut, words * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
-        }
-        SV_CUDA(cudaStreamSynchronize(s->stream));
-        return B200SV_OK;
-    };
-    rc = run();
-    if (!inScratch) {
-        cudaFree(dOut);
+    if (own) {
+        host.resize(words);
     }
-    SV_TRY(rc);
-    const double* h = inScratch ? s->h_scratch : host.data();
+    double* h = own ? host.data() : s->h_scratch;
+    SV_TRY(with_prec(s, [&](auto r) {
+        using R = decltype(r);
+        void (*kern)(const void*, RdmArgs, double*) = (D >= 4) ? k_rdm<R, 4> : (D == 2) ? k_rdm<R, 2> : k_rdm<R, 1>;
+        // one tile: the environment split over every CTA that fits on the device at once, so the state is read once at full
+        // occupancy; several tiles: at least 2 x SMs CTAs in all
+        int perSm = 2;
+        SV_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kern, RDM_THREADS, shm));
+        const uint64_t want = (tiles == 1) ? (uint64_t)sms * std::max(perSm, 1) : (2U * sms + tiles - 1) / tiles;
+        const unsigned splits = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want, a.slabs));
+        SV_CUDA(cudaMemsetAsync(dOut, 0, words * sizeof(double), s->stream));
+        kern<<<dim3((unsigned)tiles, splits), RDM_THREADS, shm, s->stream>>>(s->amps, a, (double*)dOut);
+        return launched(s);
+    }));
+    SV_CUDA(cudaMemcpyAsync(h, dOut, words * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+    SV_CUDA(cudaStreamSynchronize(s->stream));
 
     // internal row index (bit b = sorted[b]) -> caller's index (bit p = qubits[p])
     std::vector<size_t> pos(dim);

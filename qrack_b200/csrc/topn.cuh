@@ -239,8 +239,7 @@ template <int SRC> static int topn_stats(State* s, const void* src, uint64_t cou
     SV_CUDA(cudaMemsetAsync(st, 0, 3 * sizeof(unsigned long long), s->stream));
     SV_CUDA(cudaMemsetAsync(st + 1, 0xff, sizeof(unsigned long long), s->stream));
     k_topn_stats<SRC><<<topn_grid(s, k_topn_stats<SRC>, topn_units<SRC>(count)), TOPN_THREADS, 0, s->stream>>>(src, count, st);
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
+    SV_TRY(launched(s));
     SV_CUDA(cudaMemcpyAsync(reinterpret_cast<unsigned long long*>(s->h_scratch) + TOPN_ST, st, 3 * sizeof(unsigned long long),
         cudaMemcpyDeviceToHost, s->stream));
     SV_CUDA(cudaStreamSynchronize(s->stream));
@@ -250,14 +249,9 @@ template <int SRC> static int topn_stats(State* s, const void* src, uint64_t cou
 template <int SRC> static int topn_hist(State* s, const void* src, uint64_t count, const TopnPrefix& a)
 {
     unsigned long long* h = reinterpret_cast<unsigned long long*>(s->d_scratch);
-    const size_t bytes = ((size_t)1 << a.width) * sizeof(unsigned long long);
-    SV_CUDA(cudaMemsetAsync(h, 0, bytes, s->stream));
-    k_topn_hist<SRC><<<topn_grid(s, k_topn_hist<SRC>, topn_units<SRC>(count)), TOPN_THREADS, 0, s->stream>>>(src, count, a, h);
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
-    SV_CUDA(cudaMemcpyAsync(s->h_scratch, h, bytes, cudaMemcpyDeviceToHost, s->stream));
-    SV_CUDA(cudaStreamSynchronize(s->stream));
-    return B200SV_OK;
+    return scratch_reduce(s, 1 << a.width, [&] {
+        k_topn_hist<SRC><<<topn_grid(s, k_topn_hist<SRC>, topn_units<SRC>(count)), TOPN_THREADS, 0, s->stream>>>(src, count, a, h);
+    });
 }
 
 template <int SRC>
@@ -267,13 +261,11 @@ static int topn_collect(State* s, const void* src, uint64_t count, const TopnPre
     unsigned long long* ctr = reinterpret_cast<unsigned long long*>(s->d_scratch) + TOPN_CTR;
     k_topn_collect<SRC><<<topn_grid(s, k_topn_collect<SRC>, topn_units<SRC>(count)), TOPN_THREADS, 0, s->stream>>>(
         src, count, a, out, outCap, cand, candCap, ctr);
-    SV_CUDA(cudaGetLastError());
-    s->stats.kernel_launches++;
-    return B200SV_OK;
+    return launched(s);
 }
 
-// The selection proper (the state is non-zero and flushed; 1 <= n <= 2^nq).  Device buffers beyond the scratch go to *owned.
-static int topn_select(State* s, uint64_t n, uint64_t* perms, void** owned)
+// perms[0..n) = the n most probable basis states (the state is non-zero and flushed; 1 <= n <= 2^nq)
+static int topn_select(State* s, uint64_t n, uint64_t* perms)
 {
     const int state = (s->prec == 32) ? 0 : 1;
     const uint64_t dim = s->dim();
@@ -310,19 +302,13 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms, void** owned)
     uint64_t scount = dim;
     TopnEntry *dOut = nullptr, *dCand = nullptr;
     uint64_t candCap = 0U;
+    DevBuf<> owned;
     // out (and the candidates) in the scratch up to 1 MiB, else in a buffer for this call only; the counters start at 0
     auto alloc = [&](uint64_t nCand) -> int {
-        const size_t bytes = (size_t)(outCap + nCand) * sizeof(TopnEntry);
-        TopnEntry* base;
-        if (TOPN_HEAD * sizeof(unsigned long long) + bytes <= ((size_t)1 << 20)) {
-            SV_TRY(ensure_scratch(s, TOPN_HEAD + bytes / sizeof(double)));
-            base = reinterpret_cast<TopnEntry*>(reinterpret_cast<unsigned long long*>(s->d_scratch) + TOPN_HEAD);
-        } else {
-            SV_CUDA(cudaMalloc(owned, bytes));
-            base = reinterpret_cast<TopnEntry*>(*owned);
-        }
-        dOut = base;
-        dCand = nCand ? base + outCap : nullptr;
+        void* base = nullptr;
+        SV_TRY(scratch_or_own(s, TOPN_HEAD, (size_t)(outCap + nCand) * sizeof(TopnEntry), owned, &base));
+        dOut = static_cast<TopnEntry*>(base);
+        dCand = nCand ? dOut + outCap : nullptr;
         candCap = nCand;
         SV_CUDA(cudaMemsetAsync(reinterpret_cast<unsigned long long*>(s->d_scratch) + TOPN_CTR, 0, 2 * sizeof(unsigned long long),
             s->stream));
@@ -380,9 +366,8 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms, void** owned)
                                : topn_collect<2>(s, sp, scount, a, dOut, outCap, nullptr, 0));
 
     std::vector<TopnEntry> pageable;
-    const bool inScratch = !*owned;
-    TopnEntry* h = inScratch ? reinterpret_cast<TopnEntry*>(reinterpret_cast<unsigned long long*>(s->h_scratch) + TOPN_HEAD) : nullptr;
-    if (!inScratch) {
+    TopnEntry* h = owned ? nullptr : reinterpret_cast<TopnEntry*>(reinterpret_cast<unsigned long long*>(s->h_scratch) + TOPN_HEAD);
+    if (owned) {
         pageable.resize(outCap);
         h = pageable.data();
     }
@@ -402,17 +387,6 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms, void** owned)
         perms[t] = h[t].i;
     }
     return B200SV_OK;
-}
-
-// perms[0..n) = the n most probable basis states (state non-zero and flushed, 1 <= n <= 2^nq)
-static int launch_topn(State* s, uint64_t n, uint64_t* perms)
-{
-    void* owned = nullptr;
-    const int rc = topn_select(s, n, perms, &owned);
-    if (owned) {
-        cudaFree(owned);
-    }
-    return rc;
 }
 
 } // namespace b200sv

@@ -215,21 +215,25 @@ def dyadic_state(n, probs_at, prec):
 @pytest.mark.parametrize("n", [12, 13, 15, 17])
 def test_sample_exact_boundaries(n, prec):
     """b200sv_sample and b200sv_sample_many against MAll's rule: 2^14-amplitude chunks (one chunk below 15 qubits), leading
-    and trailing all-zero chunks, rnd equal to a prefix sum, rnd close to 1 over a zero tail, the FP_NORM_EPSILON early exit
-    (which fires for fp32 when the prefix comes within 2^-25 of 1) and the all-zero state."""
+    and trailing all-zero chunks, rnd equal to a prefix sum, rnd close to 1 over a zero tail, rnd above the total of an
+    unnormalised state, the FP_NORM_EPSILON early exit (which fires for fp32 when the prefix comes within 2^-25 of 1) and the
+    all-zero state."""
     s = 1 << (n - 3)        # at 17 qubits: chunks 1-3 hold the first case, chunk 0 and chunks 4-7 are empty
     t = 1 << (n - 2)
     cases = [
         {s + 4: 2, s + 6: 3, 2 * s + 2: 3, 3 * s: 1},                     # 1/4, 1/8, 1/8, 1/2 after a zero lead
         # 2^-1 .. 2^-25, then 2^-25 at the end: even indices only, so no fp32 pair sum needs more than 24 bits
         dict([(2 * i + (t if i > 12 else 0), i + 1) for i in range(25)] + [(3 * t + 2, 25)]),
+        # total 1/2: rnd 0.5 and 0.6 exceed every prefix, so the search ends at the last nonzero index
+        {s + 4: 2, 3 * s: 3, 3 * s + 2: 3},
     ]
     for probs_at in cases:
         st = dyadic_state(n, probs_at, prec)
         q = engine(n, prec, st)
         psi = q.GetQuantumState()
         cum = sorted({float(c) for c in np.cumsum(npref.probs(psi)[sorted(probs_at)])})
-        rnds = [0.0, 0.1, 0.9999999, 1 - 2.0 ** -26, 1 - 2.0 ** -40] + cum[:-1] + [math.nextafter(c, 0) for c in cum[:-1]]
+        rnds = [0.0, 0.1, 0.5, 0.6, 0.9999999, 1 - 2.0 ** -26, 1 - 2.0 ** -40]
+        rnds += cum[:-1] + [math.nextafter(c, 0) for c in cum[:-1]]
         want = [npref.sample(psi, r, prec) for r in rnds]
         got = [q.be.sample(r) for r in rnds]
         assert got == want, (probs_at, rnds, got, want)
