@@ -48,6 +48,18 @@ protected:
     /// drops PauliI as the reference's loop does (some survive it and count as PauliZ); false when a qubit is out of bounds or
     /// repeated (the base class then throws what it throws)
     bool PauliMasks(std::vector<bitLenInt>& bits, const std::vector<Pauli>& paulis, uint64_t& x, uint64_t& z) const;
+    /// the Floats query of ExpVarUnitaryAll on the state with mats[4p .. 4p + 3] applied to bits[p], read-only
+    real1_f BasisMoments(bool isExp, const std::vector<bitLenInt>& bits, const complex* mats, std::vector<real1_f> eigenVals);
+
+    // ExpVarUnitaryAll (qinterface.cpp:478-540) applies a basis gate to every listed qubit, runs the Floats query and applies
+    // the gates again: five state passes.  Here the query is one read-only sweep over the transformed blocks
+    // (b200sv_moments_basis).  The matrix form leaves the state untouched.  The U3 form then applies U(theta, phi, lambda)
+    // U(-theta, -phi, -lambda) as one gate per qubit: the reference's undo is not the inverse of its first gate, and this keeps
+    // its post-state.  More than B200SV_BASIS_MAX_QUBITS qubits go to the base class.
+    real1_f ExpVarUnitaryAll(bool isExp, const std::vector<bitLenInt>& bits, const std::vector<std::shared_ptr<complex>>& basisOps,
+        std::vector<real1_f> eigenVals = {}) override;
+    real1_f ExpVarUnitaryAll(bool isExp, const std::vector<bitLenInt>& bits, const std::vector<real1_f>& basisOps,
+        std::vector<real1_f> eigenVals = {}) override;
 
 public:
     /// 1 / OclMemDenom of device memory is the most a single state vector should take (test/benchmarks_main.cpp:288)
@@ -133,8 +145,8 @@ public:
     real1_f FirstNonzeroPhase() override { return IsZeroAmplitude() ? ZERO_R1_F : QInterface::FirstNonzeroPhase(); }
     real1_f GetExpectation(bitLenInt valueStart, bitLenInt valueLength) override;
     // The QInterface defaults ask ProbAll(i) — one device round trip — for every basis state (qinterface.cpp:478-800); here a
-    // k >= 2 query is one read-only sweep (two for VarianceBitsFactorized).  ExpectationBitsAll / VarianceBitsAll, the
-    // *UnitaryAll and the *Rdm forms reach these through QInterface's own virtual calls.
+    // k >= 2 query is one read-only sweep (two for VarianceBitsFactorized).  ExpectationBitsAll / VarianceBitsAll and the
+    // *Rdm forms reach these through QInterface's own virtual calls; the *UnitaryAll forms reach ExpVarUnitaryAll above.
     real1_f ExpectationBitsFactorized(
         const std::vector<bitLenInt>& bits, const std::vector<bitCapInt>& perms, const bitCapInt& offset = ZERO_BCI) override;
     real1_f VarianceBitsFactorized(

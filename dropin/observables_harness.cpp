@@ -12,13 +12,17 @@
 //   ExpectationBitsFactorized|VarianceBitsFactorized <cs> offset perm0 .. perm{2n-1}
 //   ExpectationFloatsFactorized|VarianceFloatsFactorized <cs> weight0 .. weight{2n-1}
 //   ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}
-//   ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..
+//   ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 .. [eigenvalue0 .. eigenvalue{2n-1}]
+//   ExpectationMatrixAll|VarianceMatrixAll <cs> <8 doubles per qubit: m00, m01, m10, m11 as re, im> [eigenvalues]
+//                                         (the matrix form of ExpectationUnitaryAll / VarianceUnitaryAll)
 //   GetReducedDensityMatrix <cs>          (prints the 2 4^n values of rho row-major, interleaved re / im)
 //   HighestProbAllN n                     (prints the n most probable basis states, QInterface::HighestProbAll(n))
 //   LossySave path p b | LossyLoad path  (LossySaveStateVector / LossyLoadStateVector)
 #include "qfactory.hpp"
 
+#include <algorithm>
 #include <cstdio>
+#include <memory>
 #include <cstdlib>
 #include <fstream>
 #include <sstream>
@@ -149,11 +153,29 @@ int main(int argc, char** argv)
                 r = q->ExpectationFloatsFactorized(bits, w);
             } else if (op == "VarianceFloatsFactorized") {
                 r = q->VarianceFloatsFactorized(bits, w);
-            } else if (op == "ExpectationUnitaryAll") {
-                r = q->ExpectationUnitaryAll(bits, w);
             } else {
-                r = q->VarianceUnitaryAll(bits, w);
+                // past the 3 angles per qubit: the eigenvalues
+                const size_t na = std::min(w.size(), 3U * bits.size());
+                const std::vector<real1_f> angles(w.begin(), w.begin() + na), eig(w.begin() + na, w.end());
+                r = (op[0] == 'E') ? q->ExpectationUnitaryAll(bits, angles, eig) : q->VarianceUnitaryAll(bits, angles, eig);
             }
+        } else if (op == "ExpectationMatrixAll" || op == "VarianceMatrixAll") {
+            std::vector<std::shared_ptr<complex>> mats;
+            for (int i = 0; i < k; ++i) {
+                std::shared_ptr<complex> m(new complex[4U], std::default_delete<complex[]>());
+                for (int e = 0; e < 4; ++e) {
+                    double re, im;
+                    ts >> re >> im;
+                    m.get()[e] = complex((real1)re, (real1)im);
+                }
+                mats.push_back(m);
+            }
+            double v;
+            std::vector<real1_f> eig;
+            while (ts >> v) {
+                eig.push_back((real1_f)v);
+            }
+            r = (op[0] == 'E') ? q->ExpectationUnitaryAll(bits, mats, eig) : q->VarianceUnitaryAll(bits, mats, eig);
         } else if (op == "ExpectationPauliAll" || op == "VariancePauliAll") {
             int v;
             std::vector<Pauli> ps;

@@ -1034,6 +1034,105 @@ real1_f QEngineCUDA::VariancePauliAll(std::vector<bitLenInt> bits, std::vector<P
     return (real1_f)(o[1] - (double)mean * o[0]);
 }
 
+// the matrix QInterface::U builds (rotational.cpp:18-26), rounded as it rounds
+static void UMatrix(real1_f theta, real1_f phi, real1_f lambda, complex* m)
+{
+    const real1 cos0 = (real1)cos(theta / 2);
+    const real1 sin0 = (real1)sin(theta / 2);
+    m[0U] = complex(cos0, ZERO_R1);
+    m[1U] = sin0 * complex((real1)(-cos(lambda)), (real1)(-sin(lambda)));
+    m[2U] = sin0 * complex((real1)cos(phi), (real1)sin(phi));
+    m[3U] = cos0 * complex((real1)cos(phi + lambda), (real1)sin(phi + lambda));
+}
+
+real1_f QEngineCUDA::BasisMoments(
+    bool isExp, const std::vector<bitLenInt>& bits, const complex* mats, std::vector<real1_f> eigenVals)
+{
+    const size_t k = bits.size();
+    if (eigenVals.empty()) {
+        for (size_t i = 0U; i < k; ++i) {
+            eigenVals.push_back(ONE_R1_F);
+            eigenVals.push_back(-ONE_R1_F);
+        }
+    }
+    // the checks of the Floats query the reference runs (qinterface.cpp:620-630, 771-780)
+    const std::string what = isExp ? "ExpectationFloatsFactorized" : "VarianceFloatsFactorized";
+    if (eigenVals.size() < (k << 1U)) {
+        throw std::invalid_argument("QInterface::" + what + "() must supply at least twice as many weights as bits!");
+    }
+    ThrowIfQbIdArrayIsBad(
+        bits, qubitCount, "QInterface::" + what + "() parameter qubits vector values must be within allocated qubit bounds!");
+    if (doNormalize) {
+        NormalizeState();
+    }
+    std::vector<int> b(bits.begin(), bits.end());
+    std::vector<double> m(k << 3U);
+    for (size_t i = 0U; i < (k << 2U); ++i) {
+        m[i << 1U] = (double)real(mats[i]);
+        m[(i << 1U) | 1U] = (double)imag(mats[i]);
+    }
+    double o[3];
+    if (k == 1U) {
+        // the Floats query's 1-bit branch on Prob(bits[0]) of the rotated state: a sweep with weights (0, 1)
+        const double w01[2]{ 0.0, 1.0 };
+        Check(b200sv_moments_basis(sv, 1, b.data(), m.data(), w01, 0.0, o));
+        const real1_f prob = clampProb((real1_f)o[1]);
+        const real1_f mean = eigenVals[0U] * (ONE_R1_F - prob) + eigenVals[1U] * prob;
+        if (isExp) {
+            return mean;
+        }
+        const real1_f var0 = eigenVals[0U] - mean;
+        const real1_f var1 = eigenVals[1U] - mean;
+        return var0 * var0 * (ONE_R1_F - prob) + var1 * var1 * prob;
+    }
+    std::vector<double> w(eigenVals.begin(), eigenVals.begin() + (k << 1U));
+    Check(b200sv_moments_basis(sv, (int)k, b.data(), m.data(), w.data(), 0.0, o));
+    const real1_f mean = (real1_f)o[1];
+    // the reference's k >= 2 variance is the unsquared sum p (w - mean) (qinterface.cpp:653)
+    return isExp ? mean : (real1_f)(o[1] - (double)mean * o[0]);
+}
+
+real1_f QEngineCUDA::ExpVarUnitaryAll(bool isExp, const std::vector<bitLenInt>& bits,
+    const std::vector<std::shared_ptr<complex>>& basisOps, std::vector<real1_f> eigenVals)
+{
+    if (bits.size() > B200SV_BASIS_MAX_QUBITS) {
+        return QEngine::ExpVarUnitaryAll(isExp, bits, basisOps, eigenVals);
+    }
+    if (bits.empty()) {
+        return ONE_R1_F;
+    }
+    std::vector<complex> mats(bits.size() << 2U);
+    for (size_t i = 0U; i < bits.size(); ++i) {
+        inv2x2(basisOps[i].get(), mats.data() + (i << 2U));
+    }
+    return BasisMoments(isExp, bits, mats.data(), eigenVals);
+}
+
+real1_f QEngineCUDA::ExpVarUnitaryAll(
+    bool isExp, const std::vector<bitLenInt>& bits, const std::vector<real1_f>& basisOps, std::vector<real1_f> eigenVals)
+{
+    if (bits.size() > B200SV_BASIS_MAX_QUBITS) {
+        return QEngine::ExpVarUnitaryAll(isExp, bits, basisOps, eigenVals);
+    }
+    if (bits.empty()) {
+        return ONE_R1_F;
+    }
+    std::vector<complex> mats(bits.size() << 2U);
+    for (size_t i = 0U; i < bits.size(); ++i) {
+        const size_t i3 = 3U * i;
+        UMatrix(-basisOps[i3], -basisOps[i3 + 1U], -basisOps[i3 + 2U], mats.data() + (i << 2U));
+    }
+    const real1_f toRet = BasisMoments(isExp, bits, mats.data(), eigenVals);
+    for (size_t i = 0U; i < bits.size(); ++i) {
+        const size_t i3 = 3U * i;
+        complex undo[4U], net[4U];
+        UMatrix(basisOps[i3], basisOps[i3 + 1U], basisOps[i3 + 2U], undo);
+        mul2x2(undo, mats.data() + (i << 2U), net);
+        Mtrx(net, bits[i]);
+    }
+    return toRet;
+}
+
 void QEngineCUDA::GetReducedDensityMatrix(const std::vector<bitLenInt>& qubits, complex* outputState)
 {
     std::vector<bool> seen(qubitCount, false);

@@ -159,6 +159,18 @@ int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, doubl
  * cannot be had. */
 #define B200SV_RDM_MAX_QUBITS 14
 int b200sv_reduced_density_matrix(b200sv_t s, int k, const int* qubits, double* out);
+/* Weighted moments in a per-qubit basis (ExpVarUnitaryAll, qinterface.cpp:478-540): with A_p the 2x2 matrix mats8[8p .. 8p + 7]
+ * (m00, m01, m10, m11, each re, im) on qubit bits[p], phi = (A_0 (x) .. (x) A_{k-1} on those qubits) psi, and
+ * out = the three moments of b200sv_moments_floats above computed on phi instead of psi: out[0] = sum |phi_i|^2,
+ * out[1] = sum |phi_i|^2 (w_i - center), out[2] = sum |phi_i|^2 (w_i - center)^2, w_i = prod_p weights[2p + bit(i, bits[p])].
+ * What the reference gets by applying A_p (the inverse of the caller's basis matrix, or U(-theta, -phi, -lambda)) to every
+ * listed qubit, running the Floats query and applying the gates again — here without writing the state.  Queued gates are
+ * flushed; the state and the memoised Prob marginals are kept; the zero state returns zeros without a launch.
+ * B200SV_EINVAL when k < 1, k > B200SV_BASIS_MAX_QUBITS (12), bits / mats8 / weights / out is NULL, or a qubit is outside
+ * [0, n) or repeated. */
+#define B200SV_BASIS_MAX_QUBITS 12
+int b200sv_moments_basis(b200sv_t s, int k, const int* bits, const double* mats8, const double* weights, double center,
+    double* out);
 /* index of the largest |psi|^2 (HighestProbAll :1995-2024) */
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm);
 /* The n most probable basis states (HighestProbAll(n), qinterface.cpp:962-1003): perms_out[0..n) sorted by

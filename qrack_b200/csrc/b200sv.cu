@@ -1500,6 +1500,7 @@ static int flush_queue(State* s)
 #include "alu_kernels.cuh"
 #include "observables.cuh"
 #include "rdm.cuh"
+#include "basis.cuh"
 #include "topn.cuh"
 #include "lossy.cuh"
 
@@ -2973,6 +2974,22 @@ int b200sv_reduced_density_matrix(b200sv_t s, int k, const int* qubits, double* 
         });
     }
     return launch_rdm(s, k, qubits, out);
+}
+
+int b200sv_moments_basis(b200sv_t s, int k, const int* bits, const double* mats8, const double* weights, double center,
+    double* out)
+{
+    SV_ENTER_RO(s);
+    if (k < 1 || k > B200SV_BASIS_MAX_QUBITS || !bits || !mats8 || !weights || !out) {
+        return einval("moments_basis: k out of range or a NULL argument");
+    }
+    SV_TRY(check_qubit_list(s, k, bits, "moments_basis: qubit index out of bounds", "moments_basis: repeated qubit"));
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        out[0] = out[1] = out[2] = 0;
+        return B200SV_OK;
+    }
+    return launch_moments_basis(s, k, bits, mats8, weights, center, out);
 }
 
 int b200sv_highest_prob(b200sv_t s, uint64_t* perm)

@@ -36,7 +36,10 @@ Grammar (tokens are whitespace separated; ``<m8>`` = 8 reals = 4 complex row-maj
     ExpectationBitsFactorized|VarianceBitsFactorized <cs> offset perm0 .. perm{2n-1}
     ExpectationFloatsFactorized|VarianceFloatsFactorized <cs> weight0 .. weight{2n-1}
     ExpectationPauliAll|VariancePauliAll <cs> pauli0 .. pauli{n-1}        (0 = I, 1 = X, 2 = Z, 3 = Y: include/pauli.hpp)
-    ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 ..  (the U3 form of ExpVarUnitaryAll)
+    ExpectationUnitaryAll|VarianceUnitaryAll <cs> theta0 phi0 lambda0 .. [eigenvalue0 .. eigenvalue{2n-1}]
+                                      (the U3 form of ExpVarUnitaryAll)
+    ExpectationMatrixAll|VarianceMatrixAll <cs> <m8 per qubit> [eigenvalues]   (its matrix form: ExpectationUnitaryAll /
+                                      VarianceUnitaryAll with one 2x2 matrix per qubit)
     GetReducedDensityMatrix <cs>      (the 2 4^n values of rho row-major, interleaved re / im; bit p of a row is qubit p of <cs>)
     HighestProbAllN n                 (the n most probable basis states, most probable first: QInterface::HighestProbAll(n))
 """
@@ -50,7 +53,8 @@ QUERY_OPS = {
     "Prob", "ProbAll", "ProbReg", "ProbMask", "ProbParity", "CProb", "ACProb", "GetAmplitude", "SumSqrDiff", "Norm",
     "ExpectationBitsAll", "VarianceBitsAll", "ExpectationBitsFactorized", "VarianceBitsFactorized",
     "ExpectationFloatsFactorized", "VarianceFloatsFactorized", "ExpectationPauliAll", "VariancePauliAll",
-    "ExpectationUnitaryAll", "VarianceUnitaryAll", "GetReducedDensityMatrix", "HighestProbAllN",
+    "ExpectationUnitaryAll", "VarianceUnitaryAll", "ExpectationMatrixAll", "VarianceMatrixAll", "GetReducedDensityMatrix",
+    "HighestProbAllN",
 }
 
 
@@ -230,9 +234,22 @@ def run(text: str, make_reg: Callable[[int, int], object]) -> Tuple[Dict[int, ob
         elif op in ("ExpectationBitsFactorized", "VarianceBitsFactorized"):
             c, p = _qubits(t, 1)
             results.append((op, (getattr(q, op)(c, [int(x) for x in t[p + 1:]], int(t[p])),)))
-        elif op in ("ExpectationFloatsFactorized", "VarianceFloatsFactorized", "ExpectationUnitaryAll", "VarianceUnitaryAll"):
+        elif op in ("ExpectationFloatsFactorized", "VarianceFloatsFactorized"):
             c, p = _qubits(t, 1)
             results.append((op, (getattr(q, op)(c, [float(x) for x in t[p:]]),)))
+        elif op in ("ExpectationUnitaryAll", "VarianceUnitaryAll"):
+            c, p = _qubits(t, 1)
+            v = [float(x) for x in t[p:]]
+            if len(v) > 3 * len(c):  # past the 3 angles per qubit: the eigenvalues
+                results.append((op, (getattr(q, op)(c, v[:3 * len(c)], v[3 * len(c):]),)))
+            else:
+                results.append((op, (getattr(q, op)(c, v),)))
+        elif op in ("ExpectationMatrixAll", "VarianceMatrixAll"):
+            c, p = _qubits(t, 1)
+            v = [float(x) for x in t[p:]]
+            mats = [[complex(v[8 * i + 2 * e], v[8 * i + 2 * e + 1]) for e in range(4)] for i in range(len(c))]
+            fn = q.ExpectationUnitaryAll if op[0] == "E" else q.VarianceUnitaryAll
+            results.append((op, (fn(c, mats, v[8 * len(c):]),)))
         elif op in ("ExpectationPauliAll", "VariancePauliAll"):
             c, p = _qubits(t, 1)
             results.append((op, (getattr(q, op)(c, [int(x) for x in t[p:]]),)))

@@ -532,7 +532,7 @@ class _ShardedBackend:
         return res
 
     _UNSUPPORTED = ("collapse_parity", "uniform_parity_rz", "uniformly_controlled", "inner", "expectation", "moments_bits",
-                    "moments_floats", "expectation_pauli", "reduced_density_matrix", "highest_probs", "lossy_save", "lossy_load",
+                    "moments_floats", "moments_basis", "expectation_pauli", "reduced_density_matrix", "highest_probs", "lossy_save", "lossy_load",
                     "compose", "decompose", "dispose_perm", "get_page", "set_page", "copy_page", "shuffle", "copy_state", "clone")
 
     def __getattr__(self, name):
