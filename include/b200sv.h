@@ -151,6 +151,11 @@ int b200sv_moments_floats(b200sv_t s, int k, const int* bits, const double* weig
  * ExpectationPauliAll (:715-769) computes by applying H / IS.H basis gates, running the Floats sweep with weights (1, -1)
  * and undoing the gates — here without writing the state.  B200SV_EINVAL when out is NULL or a mask is >= 2^n. */
 int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, double* out);
+/* Cross-page Pauli term: with phi = the 2^n amplitudes at `partner` (same precision; a device pointer readable from s's device: another
+ * state's buffer, s's own buffer, or a peer mapping of another process's page), out[0] + i out[1] = sum_j conj(phi[j ^ x]) (-1)^popcount(j & z) psi[j]
+ * and out[2] = sum_j |psi_j|^2, every term in double.  Read-only on both buffers; queued gates of s (and a pending re-page) are flushed first.
+ * The zero state returns zeros without a launch.  B200SV_EINVAL when partner or out is NULL or a mask is >= 2^n. */
+int b200sv_expectation_pauli_pair(b200sv_t s, const void* partner, uint64_t x_mask, uint64_t z_mask, double* out);
 /* Reduced density matrix on the k qubits qubits[0..k-1] (GetReducedDensityMatrix, qinterface.cpp:886-944):
  * out[2 (i 2^k + j)] + i out[2 (i 2^k + j) + 1] = sum_e psi[i, e] conj(psi[j, e]), where bit p of i and j is
  * qubit qubits[p] (the order given, not sorted) and e runs over the other qubits.  Not normalised.

@@ -76,6 +76,7 @@ SIGNATURES = {
     "b200sv_moments_bits": [H, c_int, POINTER(c_int), POINTER(c_uint64), c_uint64, c_double, POINTER(c_double)],
     "b200sv_moments_floats": [H, c_int, POINTER(c_int), POINTER(c_double), c_double, POINTER(c_double)],
     "b200sv_expectation_pauli": [H, c_uint64, c_uint64, POINTER(c_double)],
+    "b200sv_expectation_pauli_pair": [H, c_void_p, c_uint64, c_uint64, POINTER(c_double)],
     "b200sv_reduced_density_matrix": [H, c_int, POINTER(c_int), POINTER(c_double)],
     "b200sv_moments_basis": [H, c_int, POINTER(c_int), POINTER(c_double), POINTER(c_double), c_double, POINTER(c_double)],
     "b200sv_highest_prob": [H, POINTER(c_uint64)],

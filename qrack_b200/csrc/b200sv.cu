@@ -2947,6 +2947,23 @@ int b200sv_expectation_pauli(b200sv_t s, uint64_t x_mask, uint64_t z_mask, doubl
     return launch_pauli(s, x_mask, z_mask, out);
 }
 
+int b200sv_expectation_pauli_pair(b200sv_t s, const void* partner, uint64_t x_mask, uint64_t z_mask, double* out)
+{
+    SV_ENTER_RO(s);
+    if (!partner || !out) {
+        return einval("expectation_pauli_pair: null partner or out pointer");
+    }
+    if (x_mask >= s->dim() || z_mask >= s->dim()) {
+        return einval("expectation_pauli_pair: mask out-of-bounds!");
+    }
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        out[0] = out[1] = out[2] = 0;
+        return B200SV_OK;
+    }
+    return launch_pauli_pair(s, partner, x_mask, z_mask, out);
+}
+
 int b200sv_reduced_density_matrix(b200sv_t s, int k, const int* qubits, double* out)
 {
     SV_ENTER_RO(s);

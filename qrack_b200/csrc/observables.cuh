@@ -10,7 +10,9 @@
 //   * k_pauli: <psi|P|psi> of a Pauli string P given as (x, z) masks (X on x & ~z, Y on x & z, Z on z & ~x) without the basis
 //     gates the reference applies and undoes around the Floats query: P|j> = i^|y| (-1)^popcount(j & z) |j ^ x>, so every
 //     pair (j, j ^ x) is visited once (the pairing of k_xmask) and contributes twice the real part of its term.
-// Both read each 16-byte chunk once, accumulate every term in double, and issue one atomic per CTA and output.
+//   * k_pauli_pair: the same term when the two members of a pair live in different buffers (a sharded state whose Pauli
+//     string has X or Y on a rank-bit qubit pairs this rank's page with a partner page), read-only on both.
+// All of them read each 16-byte chunk once, accumulate every term in double, and issue one atomic per CTA and output.
 // Included by b200sv.cu (same translation unit as the other kernels).
 #pragma once
 
@@ -163,6 +165,45 @@ __global__ void __launch_bounds__(256) k_pauli(const typename Cx<R>::type* __res
     block_atomic_add(im, out + 2);
 }
 
+// Cross-page Pauli term: out[0] / out[1] = Re / Im sum_j (-1)^popcount(j & z) conj(phi[j ^ x]) psi[j], out[2] = sum |psi|^2.
+// The pair (j, j ^ x) has one member in each buffer, so unlike k_pauli every j is visited and both buffers are read once.
+// fp32 works on 16-byte chunks: chunk c of psi meets chunk c ^ (x >> 1) of phi, whose two amplitudes swap when bit 0 of x is
+// set; fp64 (and a one-amplitude fp32 state) pairs amplitudes.
+template <typename R>
+__global__ void __launch_bounds__(256) k_pauli_pair(const typename Cx<R>::type* __restrict__ psi,
+    const typename Cx<R>::type* __restrict__ phi, uint64_t n, uint64_t x, uint64_t z, double* out)
+{
+    typedef typename Cx<R>::type C;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    const uint64_t gid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    double s0 = 0, re = 0, im = 0;
+    if (sizeof(R) == 4 && n >= 2) {
+        const float4* p = reinterpret_cast<const float4*>(psi);
+        const float4* q = reinterpret_cast<const float4*>(phi);
+        const uint64_t xc = x >> 1;
+        const int f = (int)(x & 1U);
+        for (uint64_t c = gid; c < (n >> 1); c += stride) {
+            const float4 u = p[c], v = q[c ^ xc];
+            const float2 a[2] = {make_float2(u.x, u.y), make_float2(u.z, u.w)};
+            const float2 b[2] = {make_float2(v.x, v.y), make_float2(v.z, v.w)};
+            s0 += norm_d(a[0]) + norm_d(a[1]);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                pauli_term(a[e], b[e ^ f], __popcll((2U * c + e) & z) & 1, re, im);
+            }
+        }
+    } else {
+        for (uint64_t i = gid; i < n; i += stride) {
+            const C a = psi[i], b = phi[i ^ x];
+            s0 += norm_d(a);
+            pauli_term(a, b, __popcll(i & z) & 1, re, im);
+        }
+    }
+    block_atomic_add(re, out);
+    block_atomic_add(im, out + 1);
+    block_atomic_add(s0, out + 2);
+}
+
 // One moments sweep (arguments already validated; the state is non-zero and flushed).  out[0..2] = S0, S1, S2.
 static int launch_moments(State* s, bool prod, int k, const int* bits, const uint64_t* perms, const double* weights,
     uint64_t offset, double center, double* out)
@@ -260,6 +301,22 @@ static int launch_pauli(State* s, uint64_t x, uint64_t z, double* out)
         out[1] = 2.0 * im;
         break;
     }
+    return B200SV_OK;
+}
+
+// One cross-page Pauli sweep (masks validated; non-zero, flushed state; partner not NULL).  out as b200sv_expectation_pauli_pair.
+static int launch_pauli_pair(State* s, const void* partner, uint64_t x, uint64_t z, double* out)
+{
+    const uint64_t n = s->dim();
+    const unsigned grid = stream_grid(s->dev, (s->prec == 32 && n >= 2) ? (n >> 1) : n, 256);
+    SV_TRY(with_prec(s, [&](auto r) {
+        using R = decltype(r);
+        typedef typename Cx<R>::type C;
+        return scratch_reduce(s, 3, [&] {
+            k_pauli_pair<R><<<grid, 256, 0, s->stream>>>((const C*)s->amps, (const C*)partner, n, x, z, s->d_scratch);
+        });
+    }));
+    memcpy(out, s->h_scratch, 3 * sizeof(double));
     return B200SV_OK;
 }
 

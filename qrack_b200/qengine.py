@@ -1783,6 +1783,14 @@ class _CudaBackend:
         self._ck(self.lib.b200sv_expectation_pauli(self.h, x_mask, z_mask, out))
         return out[0], out[1]
 
+    def expectation_pauli_pair(self, partner, x_mask, z_mask):
+        """(T, sum |psi|^2) with T = sum_j conj(phi[j ^ x]) (-1)^popcount(j & z) psi[j] and phi the state at the device
+        pointer `partner` (b200sv_expectation_pauli_pair)"""
+        import ctypes
+        out = (ctypes.c_double * 3)()
+        self._ck(self.lib.b200sv_expectation_pauli_pair(self.h, ctypes.c_void_p(partner), x_mask, z_mask, out))
+        return complex(out[0], out[1]), out[2]
+
     def reduced_density_matrix(self, qubits) -> np.ndarray:
         """rho on the listed qubits, complex128 of shape (2^k, 2^k) (b200sv_reduced_density_matrix)"""
         import ctypes
