@@ -185,6 +185,17 @@ int b200sv_highest_prob(b200sv_t s, uint64_t* perm);
  * when perms_out is NULL (n > 0) or n > 2^qubits; B200SV_ENOMEM when the device buffer (16 B per listed state, beyond 1 MiB)
  * cannot be had. */
 int b200sv_highest_probs(b200sv_t s, uint64_t n, uint64_t* perms_out);
+/* The n best basis states of HighestProbAll(n) under a caller's tie key t(i) = key_xor ^ (OR over the bits b set in i of
+ * 2^key_pos[b]), key_pos[0..qubits): keys_out[t] = t(i) of the t-th entry and probs_out[t] = its P = min(|psi_i|^2, 1) in
+ * double (fp32: (double)re^2 + (double)im^2), both zero-filled past the last P > 0.  Sorted by P descending, then t(i)
+ * ascending.  key_pos == NULL means key_pos[b] = b; with key_xor = 0 that is the order of b200sv_highest_probs.  A page of a
+ * sharded state passes its logical qubits as key_pos and its rank's logical bits (and pending inversions) as key_xor, so that
+ * its ties go to the smaller logical index.  Read-only; queued gates are flushed first; the zero state gives zeros.  n = 0
+ * does nothing once the key is checked.  B200SV_EINVAL: keys_out or probs_out NULL with n > 0; n > 2^qubits; key_bits outside
+ * [qubits, 64]; a key position negative, repeated or >= key_bits; key_xor >= 2^key_bits.  B200SV_ENOMEM as
+ * b200sv_highest_probs. */
+int b200sv_highest_probs_keyed(b200sv_t s, uint64_t n, int key_bits, const int* key_pos, uint64_t key_xor,
+    uint64_t* keys_out, double* probs_out);
 /* LossySaveStateVector (reference include/statevector_turboquant.hpp; QEngineCUDA cuda.cu:3017-3035): writes the TurboQuant
  * file of the current state to `path`, block power p (1..6), `bits` per coordinate (1..16), every block rotated by the
  * rotation of `seed`.  Bit-exact with the reference codec in plain sequential IEEE arithmetic.  Read-only: queued gates are

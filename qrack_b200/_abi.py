@@ -81,6 +81,7 @@ SIGNATURES = {
     "b200sv_moments_basis": [H, c_int, POINTER(c_int), POINTER(c_double), POINTER(c_double), c_double, POINTER(c_double)],
     "b200sv_highest_prob": [H, POINTER(c_uint64)],
     "b200sv_highest_probs": [H, c_uint64, POINTER(c_uint64)],
+    "b200sv_highest_probs_keyed": [H, c_uint64, c_int, POINTER(c_int), c_uint64, POINTER(c_uint64), POINTER(c_double)],
     "b200sv_lossy_save": [H, c_char_p, c_int, c_int, c_uint64],
     "b200sv_lossy_probe": [c_char_p, c_int, POINTER(c_int), POINTER(c_int), POINTER(c_int)],
     "b200sv_lossy_load": [H, c_char_p],

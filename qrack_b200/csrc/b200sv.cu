@@ -3062,7 +3062,42 @@ int b200sv_highest_probs(b200sv_t s, uint64_t n, uint64_t* perms_out)
         std::fill(perms_out, perms_out + n, 0U);
         return B200SV_OK;
     }
-    return topn_select(s, n, perms_out);
+    return topn_select(s, n, TopnMap{s->nq, nullptr, 0U}, perms_out, nullptr);
+}
+
+int b200sv_highest_probs_keyed(b200sv_t s, uint64_t n, int key_bits, const int* key_pos, uint64_t key_xor, uint64_t* keys_out,
+    double* probs_out)
+{
+    SV_ENTER_RO(s);
+    if (key_bits < s->nq || key_bits > 64) {
+        return einval("highest_probs_keyed: key_bits outside [qubits, 64]");
+    }
+    if (key_bits < 64 && (key_xor >> key_bits)) {
+        return einval("highest_probs_keyed: key_xor is not below 2^key_bits");
+    }
+    uint64_t seen = 0U;
+    for (int b = 0; key_pos && b < s->nq; ++b) {
+        if (key_pos[b] < 0 || key_pos[b] >= key_bits || ((seen >> key_pos[b]) & 1U)) {
+            return einval("highest_probs_keyed: a key position is repeated or outside [0, key_bits)");
+        }
+        seen |= 1ULL << key_pos[b];
+    }
+    if (!n) {
+        return B200SV_OK;
+    }
+    if (!keys_out || !probs_out) {
+        return einval("highest_probs_keyed: null out pointer");
+    }
+    if (n > s->dim()) {
+        return einval("highest_probs_keyed: n is larger than 2^qubits");
+    }
+    SV_TRY(flush_queue(s));
+    if (!s->amps) {
+        std::fill(keys_out, keys_out + n, 0U);
+        std::fill(probs_out, probs_out + n, 0.0);
+        return B200SV_OK;
+    }
+    return topn_select(s, n, TopnMap{key_bits, key_pos, key_xor}, keys_out, probs_out);
 }
 
 int b200sv_lossy_save(b200sv_t s, const char* path, int p, int bits, uint64_t seed)

@@ -17,10 +17,17 @@
 //      instead of the state.
 //   4. When the class holds exactly the entries still to take, a last k_topn_collect moves the class (and anything better not
 //      yet moved) to the output.  The host sorts the n entries.
+// The index part of the key can be a tie key t(i) = key_xor ^ (OR over the bits b set in i of 2^key_pos[b]), key_bits wide,
+// instead of i (b200sv_highest_probs_keyed: a page of a sharded state ties by its logical index).  The keyed launches (KEY) of
+// k_topn_hist / k_topn_collect stage the byte tables of the map in shared memory and look t(i) up where the prefix or an
+// output entry needs it; candidates and output entries carry t(i), so the candidate passes and the host sort are unchanged.
+// The identity map runs the unkeyed instantiations, today's kernels.
 // Included by b200sv.cu (same translation unit as the other kernels).
 #pragma once
 
 #include <algorithm>
+#include <cstring>
+#include <type_traits>
 #include <vector>
 
 namespace b200sv {
@@ -30,8 +37,11 @@ static const int TOPN_DIGIT = 11; // bits per radix digit
 static const int TOPN_BINS = 1 << TOPN_DIGIT;
 static const uint64_t TOPN_CAP = 1ULL << 20; // a prefix class this small is compacted into the candidate buffer
 // unsigned long long words of the state's scratch: [0, TOPN_BINS) histogram; then count / min / max of P > 0 and the
-// output / candidate counters; from TOPN_HEAD on the output and candidate buffers when they fit in 1 MiB
+// output / candidate counters; from TOPN_HEAD on the output and candidate buffers when they fit in 1 MiB.  A keyed select
+// puts the key tables at TOPN_HEAD and the buffers after them, from TOPN_KEY_HEAD.
 static const int TOPN_ST = TOPN_BINS, TOPN_CTR = TOPN_BINS + 3, TOPN_HEAD = TOPN_BINS + 8;
+static const int TOPN_KEY_TABS = 5; // byte tables of the tie key: 40 index bits, the widest state
+static const int TOPN_KEY_HEAD = TOPN_HEAD + TOPN_KEY_TABS * 256;
 
 struct __align__(16) TopnEntry {
     unsigned long long p; // bits of P
@@ -41,10 +51,17 @@ struct __align__(16) TopnEntry {
 // the selected prefix of the composite key and the next digit
 struct TopnPrefix {
     uint64_t hiMask, hiVal; // resolved bits of P
-    uint64_t loMask, loVal; // resolved bits of the inverted index, ~i << (64 - nq)
-    int word;               // the digit is in P (0) or in the inverted index (1)
+    uint64_t loMask, loVal; // resolved bits of the inverted tie key, ~t << (64 - kbits)
+    int word;               // the digit is in P (0) or in the inverted tie key (1)
     int shift, width;       // digit = (word >> shift) & (2^width - 1)
-    int nq;
+    int kbits;              // width of the tie key (nq for the identity)
+};
+
+// the tie key of a keyed launch: t(i) = xr ^ tab[0][i & 255] ^ tab[1][(i >> 8) & 255] ^ ..., ntab tables of 256 words
+struct TopnKey {
+    const unsigned long long* tab;
+    unsigned long long xr;
+    int ntab;
 };
 
 template <typename R> __device__ __forceinline__ uint64_t topn_pbits(R re, R im)
@@ -53,7 +70,49 @@ template <typename R> __device__ __forceinline__ uint64_t topn_pbits(R re, R im)
     return (uint64_t)__double_as_longlong(fmin(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), 1.0));
 }
 
-__device__ __forceinline__ uint64_t topn_lo(uint64_t i, int nq) { return nq ? (~i) << (64 - nq) : 0U; }
+__device__ __forceinline__ uint64_t topn_lo(uint64_t i, int kbits) { return kbits ? (~i) << (64 - kbits) : 0U; }
+
+// the key tables of a keyed launch, staged by topn_stage_key (dynamic shared memory of ntab * 2 KiB)
+__device__ __forceinline__ unsigned long long* topn_key_smem()
+{
+    extern __shared__ unsigned long long topn_kt[];
+    return topn_kt;
+}
+
+// every thread of the CTA copies its share of the tables; the caller syncs before the first lookup
+__device__ __forceinline__ void topn_stage_key(const TopnKey& k)
+{
+    unsigned long long* kt = topn_key_smem();
+    for (int w = threadIdx.x; w < (k.ntab << 8); w += blockDim.x) {
+        kt[w] = k.tab[w];
+    }
+}
+
+__device__ __forceinline__ uint64_t topn_key(uint64_t i, const TopnKey& k)
+{
+    const unsigned long long* kt = topn_key_smem();
+    uint64_t t = k.xr;
+#pragma unroll
+    for (int b = 0; b < TOPN_KEY_TABS; ++b) {
+        if (b < k.ntab) {
+            t ^= kt[(b << 8) | (unsigned)((i >> (8 * b)) & 255U)]; // distinct positions: OR = XOR
+        }
+    }
+    return t;
+}
+
+// the inverted index part of the key of entry i.  Keyed: t(i) is looked up only while index bits are resolved or in the
+// digit (a.loMask or a.word), before that the index part does not take part in any comparison.
+template <bool KEY> __device__ __forceinline__ uint64_t topn_lo_of(uint64_t i, const TopnPrefix& a, const TopnKey& k)
+{
+    if constexpr (KEY) {
+        if (!a.loMask && a.word == 0) {
+            return 0U;
+        }
+        i = topn_key(i, k);
+    }
+    return topn_lo(i, a.kbits);
+}
 
 // 1: the key is better than the prefix, 0: it is in the prefix class, -1: worse
 __device__ __forceinline__ int topn_cmp(uint64_t p, uint64_t lo, const TopnPrefix& a)
@@ -154,19 +213,23 @@ __global__ void __launch_bounds__(TOPN_THREADS) k_topn_stats(const void* __restr
 }
 
 // hist[d] += the number of entries with P > 0 in the prefix class whose next digit is d
-template <int SRC>
+template <int SRC, bool KEY>
 __global__ void __launch_bounds__(TOPN_THREADS) k_topn_hist(const void* __restrict__ src, uint64_t count, TopnPrefix a,
-    unsigned long long* hist)
+    TopnKey key, unsigned long long* hist)
 {
+    static_assert(!KEY || SRC != 2, "candidates already carry their keys");
     __shared__ unsigned int h[TOPN_BINS];
     const unsigned bins = 1U << a.width;
     for (unsigned b = threadIdx.x; b < bins; b += TOPN_THREADS) {
         h[b] = 0U;
     }
+    if constexpr (KEY) {
+        topn_stage_key(key);
+    }
     __syncthreads();
     const unsigned lane = threadIdx.x & 31;
     topn_for_entries<SRC>(src, count, [&](uint64_t p, uint64_t i) {
-        const uint64_t lo = topn_lo(i, a.nq);
+        const uint64_t lo = topn_lo_of<KEY>(i, a, key);
         const bool in = p != 0U && topn_cmp(p, lo, a) == 0;
         if (!__any_sync(0xffffffffu, in)) {
             return;
@@ -208,24 +271,36 @@ __device__ __forceinline__ void topn_push(bool take, TopnEntry* buf, unsigned lo
 }
 
 // entries better than the prefix -> out; the prefix class -> cand, or to out when cand is null.  ctr[0] / ctr[1] count them.
-template <int SRC>
+// Both take the entry's tie key in place of its index.
+template <int SRC, bool KEY>
 __global__ void __launch_bounds__(TOPN_THREADS) k_topn_collect(const void* __restrict__ src, uint64_t count, TopnPrefix a,
-    TopnEntry* out, unsigned long long outCap, TopnEntry* cand, unsigned long long candCap, unsigned long long* ctr)
+    TopnKey key, TopnEntry* out, unsigned long long outCap, TopnEntry* cand, unsigned long long candCap, unsigned long long* ctr)
 {
+    static_assert(!KEY || SRC != 2, "candidates already carry their keys");
+    if constexpr (KEY) {
+        topn_stage_key(key);
+        __syncthreads();
+    }
     topn_for_entries<SRC>(src, count, [&](uint64_t p, uint64_t i) {
-        const int c = p ? topn_cmp(p, topn_lo(i, a.nq), a) : -1;
-        topn_push(c > 0 || (c == 0 && !cand), out, ctr, outCap, p, i);
+        const int c = p ? topn_cmp(p, topn_lo_of<KEY>(i, a, key), a) : -1;
+        const bool toOut = c > 0 || (c == 0 && !cand), toCand = cand && c == 0;
+        if constexpr (KEY) {
+            if (__any_sync(0xffffffffu, toOut || toCand)) { // only entries that are written need their key
+                i = topn_key(i, key);
+            }
+        }
+        topn_push(toOut, out, ctr, outCap, p, i);
         if (cand) {
-            topn_push(c == 0, cand, ctr + 1, candCap, p, i);
+            topn_push(toCand, cand, ctr + 1, candCap, p, i);
         }
     });
 }
 
-template <typename K> static unsigned topn_grid(State* s, K kern, uint64_t units)
+template <typename K> static unsigned topn_grid(State* s, K kern, uint64_t units, size_t smem = 0)
 {
     // a persistent grid: every CTA resident at once, none idle on a small source
     int perSm = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kern, TOPN_THREADS, 0);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, kern, TOPN_THREADS, smem);
     const uint64_t need = (units + TOPN_THREADS - 1) / TOPN_THREADS;
     return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(need, (uint64_t)sm_count(s->dev) * std::max(perSm, 1)));
 }
@@ -246,42 +321,103 @@ template <int SRC> static int topn_stats(State* s, const void* src, uint64_t cou
     return B200SV_OK;
 }
 
-template <int SRC> static int topn_hist(State* s, const void* src, uint64_t count, const TopnPrefix& a)
+template <bool KEY> static size_t topn_smem(const TopnKey& k) { return KEY ? (size_t)k.ntab * 256 * sizeof(unsigned long long) : 0; }
+
+template <int SRC, bool KEY> static int topn_hist(State* s, const void* src, uint64_t count, const TopnPrefix& a, const TopnKey& k)
 {
     unsigned long long* h = reinterpret_cast<unsigned long long*>(s->d_scratch);
+    const size_t smem = topn_smem<KEY>(k);
     return scratch_reduce(s, 1 << a.width, [&] {
-        k_topn_hist<SRC><<<topn_grid(s, k_topn_hist<SRC>, topn_units<SRC>(count)), TOPN_THREADS, 0, s->stream>>>(src, count, a, h);
+        k_topn_hist<SRC, KEY><<<topn_grid(s, k_topn_hist<SRC, KEY>, topn_units<SRC>(count), smem), TOPN_THREADS, smem, s->stream>>>(
+            src, count, a, k, h);
     });
 }
 
-template <int SRC>
-static int topn_collect(State* s, const void* src, uint64_t count, const TopnPrefix& a, TopnEntry* out, uint64_t outCap,
-    TopnEntry* cand, uint64_t candCap)
+template <int SRC, bool KEY>
+static int topn_collect(State* s, const void* src, uint64_t count, const TopnPrefix& a, const TopnKey& k, TopnEntry* out,
+    uint64_t outCap, TopnEntry* cand, uint64_t candCap)
 {
     unsigned long long* ctr = reinterpret_cast<unsigned long long*>(s->d_scratch) + TOPN_CTR;
-    k_topn_collect<SRC><<<topn_grid(s, k_topn_collect<SRC>, topn_units<SRC>(count)), TOPN_THREADS, 0, s->stream>>>(
-        src, count, a, out, outCap, cand, candCap, ctr);
+    const size_t smem = topn_smem<KEY>(k);
+    k_topn_collect<SRC, KEY><<<topn_grid(s, k_topn_collect<SRC, KEY>, topn_units<SRC>(count), smem), TOPN_THREADS, smem,
+        s->stream>>>(src, count, a, k, out, outCap, cand, candCap, ctr);
     return launched(s);
 }
 
-// perms[0..n) = the n most probable basis states (the state is non-zero and flushed; 1 <= n <= 2^nq)
-static int topn_select(State* s, uint64_t n, uint64_t* perms)
+// f(SRC, KEY) as std::integral_constants: the source (0 / 1: an fp32 / fp64 state, 2: candidates) and whether t(i) is looked
+// up (a keyed select on the state; candidates carry their keys)
+template <typename F> static int topn_dispatch(int src, bool keyed, F&& f)
+{
+    using S0 = std::integral_constant<int, 0>;
+    using S1 = std::integral_constant<int, 1>;
+    if (src == 2) {
+        return f(std::integral_constant<int, 2>(), std::false_type());
+    }
+    if (keyed) {
+        return src == 0 ? f(S0(), std::true_type()) : f(S1(), std::true_type());
+    }
+    return src == 0 ? f(S0(), std::false_type()) : f(S1(), std::false_type());
+}
+
+// The tie key of a select: t(i) = xr ^ (OR over the bits b set in i of 2^pos[b]), `bits` wide.  pos == nullptr means
+// pos[b] = b; with that and xr == 0 the select runs the unkeyed kernels.
+struct TopnMap {
+    int bits;
+    const int* pos;
+    uint64_t xr;
+};
+
+// keys[0..n) = the tie keys of the n most probable basis states, probs[0..n) their P when probs is not null (the state is
+// non-zero and flushed; 1 <= n <= 2^nq; the map was checked by the caller)
+static int topn_select(State* s, uint64_t n, const TopnMap& map, uint64_t* keys, double* probs)
 {
     const int state = (s->prec == 32) ? 0 : 1;
     const uint64_t dim = s->dim();
-    SV_TRY(ensure_scratch(s, TOPN_HEAD));
-    // pass 1: the count, smallest and largest P > 0
+    bool keyed = map.xr != 0;
+    for (int b = 0; map.pos && b < s->nq; ++b) {
+        keyed = keyed || map.pos[b] != b;
+    }
+    const size_t head = keyed ? TOPN_KEY_HEAD : TOPN_HEAD;
+    SV_TRY(ensure_scratch(s, head));
+    // pass 1: the count, smallest and largest P > 0 (the index plays no part)
     SV_TRY(state == 0 ? topn_stats<0>(s, s->amps, dim) : topn_stats<1>(s, s->amps, dim));
     const unsigned long long* hs = reinterpret_cast<const unsigned long long*>(s->h_scratch);
     const uint64_t pos = hs[TOPN_ST], pmin = hs[TOPN_ST + 1], pmax = hs[TOPN_ST + 2];
-    std::fill(perms, perms + n, 0U);
+    std::fill(keys, keys + n, 0U);
+    if (probs) {
+        std::fill(probs, probs + n, 0.0);
+    }
     if (!pos) {
         return B200SV_OK;
     }
     const uint64_t outCap = std::min(n, pos);
 
+    // the byte tables of t(i) at TOPN_HEAD of the device scratch; staged again whenever alloc grows (reallocates) the scratch
+    TopnKey key{nullptr, map.xr, (s->nq + 7) / 8};
+    std::vector<unsigned long long> tabs;
+    size_t tabsAt = 0; // the scratch size the tables were staged into
+    auto stage = [&]() -> int {
+        key.tab = reinterpret_cast<const unsigned long long*>(s->d_scratch) + TOPN_HEAD;
+        tabsAt = s->scratch_doubles;
+        SV_CUDA(cudaMemcpyAsync(const_cast<unsigned long long*>(key.tab), tabs.data(), tabs.size() * sizeof(unsigned long long),
+            cudaMemcpyHostToDevice, s->stream));
+        return B200SV_OK;
+    };
+    if (keyed) {
+        tabs.assign((size_t)key.ntab * 256, 0U);
+        for (int b = 0; b < s->nq; ++b) {
+            const uint64_t bit = 1ULL << (map.pos ? map.pos[b] : b);
+            for (unsigned v = 0; v < 256U; ++v) {
+                if ((v >> (b & 7)) & 1U) {
+                    tabs[(size_t)(b >> 3) * 256 + v] |= bit;
+                }
+            }
+        }
+        SV_TRY(stage());
+    }
+
     TopnPrefix a{};
-    a.nq = s->nq;
+    a.kbits = map.bits;
     int L = 0;         // resolved key bits (P: 0..63, then the index: 64..64 + nq - 1)
     uint64_t r = n;    // entries still to take from the prefix class
     uint64_t cls = pos; // entries in the prefix class
@@ -306,7 +442,10 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms)
     // out (and the candidates) in the scratch up to 1 MiB, else in a buffer for this call only; the counters start at 0
     auto alloc = [&](uint64_t nCand) -> int {
         void* base = nullptr;
-        SV_TRY(scratch_or_own(s, TOPN_HEAD, (size_t)(outCap + nCand) * sizeof(TopnEntry), owned, &base));
+        SV_TRY(scratch_or_own(s, head, (size_t)(outCap + nCand) * sizeof(TopnEntry), owned, &base));
+        if (keyed && s->scratch_doubles != tabsAt) {
+            SV_TRY(stage());
+        }
         dOut = static_cast<TopnEntry*>(base);
         dCand = nCand ? dOut + outCap : nullptr;
         candCap = nCand;
@@ -319,8 +458,9 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms)
         if (src != 2 && cls <= TOPN_CAP) {
             // the class fits: move it to the candidates, and what is better to the output, in one read of the state
             SV_TRY(alloc(cls));
-            SV_TRY(state == 0 ? topn_collect<0>(s, sp, scount, a, dOut, outCap, dCand, candCap)
-                              : topn_collect<1>(s, sp, scount, a, dOut, outCap, dCand, candCap));
+            SV_TRY(topn_dispatch(src, keyed, [&](auto S, auto K) {
+                return topn_collect<decltype(S)::value, decltype(K)::value>(s, sp, scount, a, key, dOut, outCap, dCand, candCap);
+            }));
             src = 2;
             sp = dCand;
             scount = cls;
@@ -332,11 +472,13 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms)
             a.shift = 64 - L - w;
         } else {
             a.word = 1;
-            w = std::min(TOPN_DIGIT, s->nq - (L - 64));
+            w = std::min(TOPN_DIGIT, a.kbits - (L - 64));
             a.shift = 64 - (L - 64) - w;
         }
         a.width = w;
-        SV_TRY(src == 0 ? topn_hist<0>(s, sp, scount, a) : src == 1 ? topn_hist<1>(s, sp, scount, a) : topn_hist<2>(s, sp, scount, a));
+        SV_TRY(topn_dispatch(src, keyed, [&](auto S, auto K) {
+            return topn_hist<decltype(S)::value, decltype(K)::value>(s, sp, scount, a, key);
+        }));
         // the bin holding the r-th remaining entry, counted from the best bin down
         const unsigned long long* cnt = reinterpret_cast<const unsigned long long*>(s->h_scratch);
         uint64_t above = 0U;
@@ -361,9 +503,9 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms)
     if (!dOut) {
         SV_TRY(alloc(0));
     }
-    SV_TRY(src == 0 ? topn_collect<0>(s, sp, scount, a, dOut, outCap, nullptr, 0)
-                    : src == 1 ? topn_collect<1>(s, sp, scount, a, dOut, outCap, nullptr, 0)
-                               : topn_collect<2>(s, sp, scount, a, dOut, outCap, nullptr, 0));
+    SV_TRY(topn_dispatch(src, keyed, [&](auto S, auto K) {
+        return topn_collect<decltype(S)::value, decltype(K)::value>(s, sp, scount, a, key, dOut, outCap, nullptr, 0);
+    }));
 
     std::vector<TopnEntry> pageable;
     TopnEntry* h = owned ? nullptr : reinterpret_cast<TopnEntry*>(reinterpret_cast<unsigned long long*>(s->h_scratch) + TOPN_HEAD);
@@ -384,7 +526,10 @@ static int topn_select(State* s, uint64_t n, uint64_t* perms)
     }
     std::sort(h, h + outCap, [](const TopnEntry& x, const TopnEntry& y) { return x.p != y.p ? x.p > y.p : x.i < y.i; });
     for (uint64_t t = 0; t < outCap; ++t) {
-        perms[t] = h[t].i;
+        keys[t] = h[t].i;
+        if (probs) {
+            std::memcpy(&probs[t], &h[t].p, sizeof(double));
+        }
     }
     return B200SV_OK;
 }

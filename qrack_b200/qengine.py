@@ -1382,6 +1382,10 @@ class QEngineHost:
             raise ValueError("QInterface::HighestProbAll(n) requested more !")
         if self.doNormalize:
             self.NormalizeState()
+        return self._highest_probs(n)
+
+    def _highest_probs(self, n: int) -> list:
+        """HighestProbAllN past its edge rules (2 <= n <= 2^qubits): the backend's select"""
         return self.be.highest_probs(n)
 
     # lossy checkpoints: the TurboQuant file of include/statevector_turboquant.hpp, encoded and decoded on the device
@@ -1812,6 +1816,21 @@ class _CudaBackend:
         out = np.zeros(max(n, 1), dtype=np.uint64)
         self._ck(self.lib.b200sv_highest_probs(self.h, n, out.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64))))
         return [int(v) for v in out[:n]]
+
+    def highest_probs_keyed(self, n: int, key_bits: int, key_pos, key_xor: int):
+        """(keys, probs): the n most probable basis states under the tie key t(i) = key_xor ^ (OR over the bits b set in i of
+        2^key_pos[b]) (None: key_pos[b] = b), as uint64 keys and their float64 P, by P descending, then key ascending,
+        zero-filled past the last P > 0 (b200sv_highest_probs_keyed)"""
+        import ctypes
+        if key_pos is not None and len(key_pos) != self.n_qubits():
+            raise ValueError("highest_probs_keyed: key_pos needs one position per qubit")
+        keys = np.zeros(max(n, 1), dtype=np.uint64)
+        probs = np.zeros(max(n, 1), dtype=np.float64)
+        pos = None if key_pos is None else (ctypes.c_int * max(len(key_pos), 1))(*key_pos)
+        self._ck(self.lib.b200sv_highest_probs_keyed(self.h, n, key_bits, pos, key_xor,
+                                                     keys.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64)),
+                                                     probs.ctypes.data_as(ctypes.POINTER(ctypes.c_double))))
+        return keys[:n], probs[:n]
 
     def lossy_save(self, path: str, p: int, bits: int, seed: int):
         """the TurboQuant file of the state (b200sv_lossy_save)"""

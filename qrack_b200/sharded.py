@@ -12,14 +12,17 @@ rank-bit qubits are per-rank scalars or predicated local phases, controls on ran
 (QPager's meta-controlled cases, ``src/qpager.cpp:452-593``), scalars (Prob, norms) are one ``all_reduce``.  The observable
 moments and Pauli strings are per-rank read-only sweeps and one ``all_reduce`` too; a Pauli string with X or Y on a rank-bit
 qubit pairs each page with one partner page, read in place or received into the spare buffer, with no exchange.
+``HighestProbAll(n)`` is a per-rank radix select whose ties go to the smaller LOGICAL index, then one ``all_gather`` of every
+rank's best min(n, page) entries and a merge.
 
 ``QEngineSharded`` derives from ``QEngineHost`` — the same gate dispatch mirror as ``QEngineCUDA`` — and supplies a
 backend whose primitives are distributed, so the gate-level ``QInterface`` methods (H, T, CNOT, MC/MAC gates, QFT, INC/DEC,
-ZeroPhaseFlip, Prob*, ForceM, M, MAll, HighestProbAll, ProbMaskAll, Expectation/Variance{BitsAll, BitsFactorized,
-FloatsFactorized, PauliAll}, ExpectationUnitaryAll past 12 qubits, …) work unchanged on top of it.  Primitives that are not
-sharded (Compose/Decompose, ForceMParity, UniformParityRZ, SumSqrDiff, the register expectation primitive, the per-qubit basis sweep behind
-ExpectationUnitaryAll up to 12 qubits, reduced density matrices, HighestProbAll(n), lossy checkpoints, the native QAlu
-sweeps, page ops) raise ``NotImplementedError`` identically on every rank.  The local engine and the communicator are injected: ``QEngineCUDA`` over a torch CUDA buffer +
+ZeroPhaseFlip, Prob*, ForceM, M, MAll, HighestProbAll, HighestProbAll(n), ProbMaskAll, Expectation/Variance{BitsAll,
+BitsFactorized, FloatsFactorized, PauliAll}, ExpectationUnitaryAll past 12 qubits, …) work unchanged on top of it.  Primitives
+that are not sharded (Compose/Decompose, ForceMParity, UniformParityRZ, SumSqrDiff, the register expectation primitive, the
+per-qubit basis sweep behind ExpectationUnitaryAll up to 12 qubits, reduced density matrices, the single-vector top-n
+primitive ``highest_probs``, lossy checkpoints, the native QAlu sweeps, page ops) raise ``NotImplementedError`` identically
+on every rank.  The local engine and the communicator are injected: ``QEngineCUDA`` over a torch CUDA buffer +
 NCCL on the GPU box; the oracle restatement over a torch CPU buffer + gloo in the CPU tests.
 """
 from __future__ import annotations
@@ -244,6 +247,15 @@ class _Gate:
     def __init__(self, t, cmask, cval, m):
         self.t, self.cmask, self.cval, self.m = t, cmask, cval, m
         self.diag = (m[1] == 0 and m[2] == 0)
+
+
+def merge_top_n(keys: np.ndarray, probs: np.ndarray, n: int) -> list:
+    """the n keys of largest P among (keys, probs) pairs, ties to the smaller key; P = 0 (and padding) never listed, the
+    list zero-filled past the last P > 0"""
+    live = probs > 0
+    keys, probs = keys[live], probs[live]
+    o = np.lexsort((keys, -probs))[:n]
+    return [int(v) for v in keys[o]] + [0] * (n - o.size)
 
 
 class _ShardedBackend:
@@ -627,6 +639,33 @@ class _ShardedBackend:
         t *= (1, 1j, -1, -1j)[bin(px & pz).count("1") & 3]
         return tuple(self._allreduce([s0, sign * t.real]))
 
+    # ---- top n: a keyed select per rank + one all_gather; nothing is written and the qubit map does not change ----------
+    def highest_probs_merged(self, n: int) -> list:
+        """HighestProbAll(n) over the pages: the n logical indices of largest P = min(|psi|^2, 1), ties to the smaller logical
+        index, zero-filled past the last P > 0; the same list on every rank.
+
+        Every rank orders its page by one key, (P desc, t asc) with t(j) = the logical index of its local index j: local
+        physical bit b is logical qubit inv[b], this rank's rank bits and the pending inversions are a constant XOR, so
+        t(j) = _logical_index((rank << nl) | j) ^ xinv, the index sample / highest_prob report.  Under a key shared by
+        every rank the global top n lies in the union of each rank's top min(n, 2^nl), so one all_gather of those (key, P)
+        pairs, zero-padded to a fixed size, and a merge give it exactly."""
+        self.flush()
+        inv = {p: q for q, p in enumerate(self.perm)}                     # physical bit -> logical qubit
+        xr = self.xinv
+        for g in range(self.k):
+            if (self.rank >> g) & 1:
+                xr ^= 1 << inv[self.nl + g]
+        m = min(n, 1 << self.nl)
+        keys, probs = self.loc.be.highest_probs_keyed(m, self.n, [inv[b] for b in range(self.nl)], xr)
+        mine = np.stack([np.asarray(keys, dtype=np.uint64).view(np.int64), np.asarray(probs, dtype=np.float64).view(np.int64)])
+        if self.world > 1:
+            torch = self.shard.torch
+            local = torch.from_numpy(np.ascontiguousarray(mine)).to(self.shard.device)
+            parts = [torch.empty_like(local) for _ in range(self.world)]
+            self.dist.all_gather(parts, local)
+            mine = torch.cat(parts, 1).cpu().numpy()
+        return merge_top_n(mine[0].view(np.uint64), mine[1].view(np.float64), n)
+
     _UNSUPPORTED = ("collapse_parity", "uniform_parity_rz", "uniformly_controlled", "inner", "expectation",
                     "moments_basis", "reduced_density_matrix", "highest_probs", "lossy_save", "lossy_load",
                     "compose", "decompose", "dispose_perm", "get_page", "set_page", "copy_page", "shuffle", "copy_state", "clone")
@@ -809,3 +848,6 @@ class QEngineSharded(QEngineHost):
 
     def flush(self):
         self.be.flush()
+
+    def _highest_probs(self, n: int) -> list:
+        return self.be.highest_probs_merged(n)

@@ -16,6 +16,7 @@ import argparse
 import json
 import os
 import random
+import re
 import subprocess
 import sys
 import time
@@ -47,7 +48,7 @@ def timed(q, fn, reps):
 
 def kernel_roles(fn, calls=3):
     """(kernels recorded, of which read the state) over `calls` calls, from the kernel names torch.profiler records: the source
-    is the template argument, 0 / 1 = an fp32 / fp64 state, 2 = the candidate buffer"""
+    is the first template argument, 0 / 1 = an fp32 / fp64 state, 2 = the candidate buffer"""
     import torch
     from torch.profiler import ProfilerActivity, profile
     torch.cuda.init()
@@ -56,7 +57,7 @@ def kernel_roles(fn, calls=3):
             fn()
         torch.cuda.synchronize()
     names = [e.name for e in prof.events() if "k_topn_" in e.name]
-    return len(names), sum(1 for s in names if "<0>" in s or "<1>" in s)
+    return len(names), sum(1 for s in names if re.search(r"<[01][,>]", s))
 
 
 def prepare(q, kind, n):
