@@ -221,6 +221,15 @@ int b200sv_sample(b200sv_t s, double rnd, uint64_t* perm);
  * the k measured bits are read off each sampled basis state — same distribution as drawing from the 2^k histogram);
  * rnds[i] in [0,1) -> perms[i] = b200sv_sample(s, rnds[i]) (MAll's search, its FP_NORM_EPSILON early exit included). */
 int b200sv_sample_many(b200sv_t s, int n_shots, const double* rnds, uint64_t* perms);
+/* The samples of b200sv_sample_many mapped through a caller's tie key t(i) = key_xor ^ (OR over the bits b set in i of
+ * 2^key_pos[b]), key_pos[0..qubits): keys_out[i] = t(b200sv_sample(s, rnds[i])).  key_pos == NULL means key_pos[b] = b.  A page
+ * of a sharded state passes its logical qubits and its rank's logical bits (and pending inversions), so its samples come back
+ * as logical indices.  Read-only; queued gates are flushed first.  The zero state gives t(2^n - 1) for every shot without a
+ * launch; any other state costs two launches (chunk sums, search) whatever n_shots is.  B200SV_EINVAL: n_shots < 0; rnds or
+ * keys_out NULL with n_shots > 0; the key as in b200sv_highest_probs_keyed (key_bits outside [qubits, 64]; a key position
+ * negative, repeated or >= key_bits; key_xor >= 2^key_bits). */
+int b200sv_sample_keyed(b200sv_t s, int n_shots, const double* rnds, int key_bits, const int* key_pos, uint64_t key_xor,
+    uint64_t* keys_out);
 
 /* ---- structure (state.cpp:1271-1748; utility.cpp:54-68) ---- */
 /* a <- a (x) b with b's qubits inserted at `start` (Compose :1368-1459; start==n_a is the append form :1271-1362) */

@@ -88,6 +88,7 @@ SIGNATURES = {
     "b200sv_lossy_rotation": [c_int, c_int, c_uint64, c_void_p],
     "b200sv_sample": [H, c_double, POINTER(c_uint64)],
     "b200sv_sample_many": [H, c_int, POINTER(c_double), POINTER(c_uint64)],
+    "b200sv_sample_keyed": [H, c_int, POINTER(c_double), c_int, POINTER(c_int), c_uint64, POINTER(c_uint64)],
     "b200sv_compose": [H, H, c_int],
     "b200sv_decompose": [H, c_int, c_int, H],
     "b200sv_dispose_perm": [H, c_int, c_int, c_uint64],

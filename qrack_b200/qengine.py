@@ -1241,8 +1241,8 @@ class QEngineHost:
         """QEngine::MultiShotMeasureMask (src/qengine/qengine.cpp:542-576): `shots` samples of the listed qubits without
         collapse, as {outcome: count} with qPowers[p] -> outcome bit p.  Few measured qubits: one histogram sweep
         (ProbBitsAll) and host draws, like the reference.  Many measured qubits (where the reference builds a 2^k histogram by
-        reading the whole state): basis states are sampled on the device (one chunk-sum sweep for all shots) and the measured
-        bits are read off them — the same distribution.  Draws come from this engine's generator (the reference seeds
+        reading the whole state): basis states are sampled on the device (one chunk-sum sweep and one search for all shots) and
+        the measured bits are read off them — the same distribution.  Draws come from this engine's generator (the reference seeds
         std::mt19937 from std::random_device: outcomes are not reproducible there either)."""
         if not shots:
             return {}
@@ -1267,12 +1267,13 @@ class QEngineHost:
             return out
         if self.doNormalize:
             self.NormalizeState()
-        perms = self.be.sample_many([self.Rand() for _ in range(shots)])
-        for perm in perms:
-            key = 0
-            for p, b in enumerate(bits):
-                key |= ((int(perm) >> b) & 1) << p
-            out[key] = out.get(key, 0) + 1
+        perms = np.asarray(self.be.sample_many([self.Rand() for _ in range(shots)]), dtype=np.uint64)
+        keys = np.zeros(perms.size, dtype=np.uint64)
+        for p, b in enumerate(bits):
+            keys |= ((perms >> np.uint64(b)) & np.uint64(1)) << np.uint64(p)
+        uniq, first, counts = np.unique(keys, return_index=True, return_counts=True)
+        for i in np.argsort(first):  # the outcomes in order of first appearance
+            out[int(uniq[i])] = int(counts[i])
         return out
 
     def CtrlOrAntiProb(self, controlState: bool, control: int, target: int) -> float:  # state.cpp:1814-1869
@@ -1853,6 +1854,20 @@ class _CudaBackend:
         out = (ctypes.c_uint64 * max(n, 1))()
         self._ck(self.lib.b200sv_sample_many(self.h, n, r, out))
         return [int(out[i]) for i in range(n)]
+
+    def sample_keyed(self, rnds, key_bits: int, key_pos, key_xor: int) -> np.ndarray:
+        """t(sample(rnd)) for every rnd as uint64, t(i) = key_xor ^ (OR over the bits b set in i of 2^key_pos[b]) (None:
+        key_pos[b] = b) (b200sv_sample_keyed)"""
+        import ctypes
+        if key_pos is not None and len(key_pos) != self.n_qubits():
+            raise ValueError("sample_keyed: key_pos needs one position per qubit")
+        r = np.ascontiguousarray(rnds, dtype=np.float64).reshape(-1)
+        keys = np.zeros(max(r.size, 1), dtype=np.uint64)
+        pos = None if key_pos is None else np.ascontiguousarray(key_pos, dtype=np.intc)
+        self._ck(self.lib.b200sv_sample_keyed(self.h, r.size, r.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), key_bits,
+                                              None if pos is None else pos.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                              key_xor, keys.ctypes.data_as(ctypes.POINTER(ctypes.c_uint64))))
+        return keys[:r.size]
 
     def compose(self, other: "_CudaBackend", start: int):
         self._ck(self.lib.b200sv_compose(self.h, other.h, start))

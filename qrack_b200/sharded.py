@@ -13,12 +13,15 @@ rank-bit qubits are per-rank scalars or predicated local phases, controls on ran
 moments and Pauli strings are per-rank read-only sweeps and one ``all_reduce`` too; a Pauli string with X or Y on a rank-bit
 qubit pairs each page with one partner page, read in place or received into the spare buffer, with no exchange.
 ``HighestProbAll(n)`` is a per-rank radix select whose ties go to the smaller LOGICAL index, then one ``all_gather`` of every
-rank's best min(n, page) entries and a merge.
+rank's best min(n, page) entries and a merge.  ``MultiShotMeasureMask`` over more than 16 qubits samples every shot as
+``MAll``'s search would: each rank searches its page on the device for the shots that land there, returning logical indices,
+and one ``all_reduce`` of a slot per shot gathers them.
 
 ``QEngineSharded`` derives from ``QEngineHost`` — the same gate dispatch mirror as ``QEngineCUDA`` — and supplies a
 backend whose primitives are distributed, so the gate-level ``QInterface`` methods (H, T, CNOT, MC/MAC gates, QFT, INC/DEC,
-ZeroPhaseFlip, Prob*, ForceM, M, MAll, HighestProbAll, HighestProbAll(n), ProbMaskAll, Expectation/Variance{BitsAll,
-BitsFactorized, FloatsFactorized, PauliAll}, ExpectationUnitaryAll past 12 qubits, …) work unchanged on top of it.  Primitives
+ZeroPhaseFlip, Prob*, ForceM, M, MAll, MultiShotMeasureMask, HighestProbAll, HighestProbAll(n), ProbMaskAll,
+Expectation/Variance{BitsAll, BitsFactorized, FloatsFactorized, PauliAll}, ExpectationUnitaryAll past 12 qubits, …) work
+unchanged on top of it.  Primitives
 that are not sharded (Compose/Decompose, ForceMParity, UniformParityRZ, SumSqrDiff, the register expectation primitive, the
 per-qubit basis sweep behind ExpectationUnitaryAll up to 12 qubits, reduced density matrices, the single-vector top-n
 primitive ``highest_probs``, lossy checkpoints, the native QAlu sweeps, page ops) raise ``NotImplementedError`` identically
@@ -247,6 +250,26 @@ class _Gate:
     def __init__(self, t, cmask, cval, m):
         self.t, self.cmask, self.cval, self.m = t, cmask, cval, m
         self.diag = (m[1] == 0 and m[2] == 0)
+
+
+def rank_walk(tots, rnds):
+    """_ShardedBackend.sample's walk over the page totals for every rnd at once: (the rank whose page it searches, the rnd
+    it passes there), the rank -1 where every page is zero.  np.cumsum adds in order, so cum holds the doubles of sample's
+    running sum (a page with total 0 adds 0.0, which changes nothing).  Past the total, the last nonzero page is searched
+    with rnd - (cum - tots[last]): the total less that page, not the sum of the pages before it."""
+    tots = np.asarray(tots, dtype=np.float64)
+    rnds = np.asarray(rnds, dtype=np.float64)
+    live = tots > 0
+    if not live.any():
+        return np.full(rnds.size, -1, dtype=np.int64), rnds.copy()
+    cum = np.cumsum(np.where(live, tots, 0.0))
+    before = np.concatenate(([0.0], cum[:-1]))
+    hit = live[None, :] & (cum[None, :] > rnds[:, None])
+    found = hit.any(axis=1)
+    last = int(np.flatnonzero(live)[-1])
+    pick = np.where(found, hit.argmax(axis=1), last).astype(np.int64)
+    res = np.where(found, rnds - before[pick], rnds - (cum[-1] - tots[last]))
+    return pick, res
 
 
 def merge_top_n(keys: np.ndarray, probs: np.ndarray, n: int) -> list:
@@ -533,6 +556,33 @@ class _ShardedBackend:
         phys = int(round(self._allreduce([idx])[0]))
         return self._logical_index(phys) ^ self.xinv
 
+    def sample_many(self, rnds) -> list:
+        """[sample(rnd) for rnd in rnds] with one search per rank: every rank walks the page totals for every rnd
+        (rank_walk), searches its own page for its shots' residual rnds, keyed so that it returns logical indices (the key
+        of highest_probs_merged), and one all_reduce of a slot per shot, filled by the rank that searched it, gives every
+        rank the list.  Nothing is written and nothing is exchanged."""
+        self.flush()
+        tots = [t[0] for t in self._gather_scalars([self.loc.be.norm(0.0)])]
+        pick, res = rank_walk(tots, rnds)
+        if pick.size and pick[0] < 0:
+            return [(1 << self.n) - 1] * pick.size
+        out = np.zeros(pick.size, dtype=np.int64)
+        mine = pick == self.rank
+        if mine.any():
+            inv = {p: q for q, p in enumerate(self.perm)}                 # physical bit -> logical qubit
+            xr = self.xinv
+            for g in range(self.k):
+                if (self.rank >> g) & 1:
+                    xr ^= 1 << inv[self.nl + g]
+            keys = self.loc.be.sample_keyed(res[mine], self.n, [inv[b] for b in range(self.nl)], xr)
+            out[mine] = np.asarray(keys, dtype=np.uint64).view(np.int64)
+        if self.world > 1:
+            torch = self.shard.torch
+            t = torch.from_numpy(out).to(self.shard.device)
+            self.dist.all_reduce(t)
+            out = t.cpu().numpy()
+        return out.tolist()
+
     def highest_prob(self) -> int:
         self.flush()
         li = self.loc.be.highest_prob()
@@ -816,7 +866,9 @@ class _ShardedBackend:
 
 
 class QEngineSharded(QEngineHost):
-    """QPager-like engine over `world` ranks; constructed collectively by every rank with the same arguments."""
+    """QPager-like engine over `world` ranks; constructed collectively by every rank with the same arguments.  Queries
+    (Prob*, MAll, MultiShotMeasureMask, HighestProbAll(n), the Expectation / Variance family) return the same value on
+    every rank, and the read-only ones leave the pages and the qubit map alone."""
 
     def __init__(self, qBitCount: int, initState: int = 0, rgp=None, phaseFac=None, doNorm: bool = False,
                  randomGlobalPhase: bool = False, precision: int = 32, dist=None, world: int = 1, rank: int = 0,
