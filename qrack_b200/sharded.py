@@ -82,6 +82,7 @@ class ShardBuffers:
 
     needs_top = True  # the all-to-all exchanges the TOP k local bits: victims must be moved there first
     min_victim_bit = 0
+    chunk_floor = 0   # local swaps bring any local qubit to the top
 
     def zero_live(self):
         self.buf.zero_()
@@ -142,13 +143,16 @@ class P2PShardBuffers:
     and stores straight into the peers' pages — no local pre-permutation, no NCCL staging."""
 
     needs_top = False
-    min_victim_bit = 8  # keep >= 2 KB contiguous runs per destination
+    min_victim_bit = 8  # keep >= 2 KB contiguous runs per destination (preferred)
+    # the re-page kernels move whole 16-byte chunks: an fp32 chunk holds qubit 0, which can never be a victim (hard floor)
+    CHUNK_FLOOR = {32: 1, 64: 0}
 
     def __init__(self, n_local: int, precision: int, device_index: int, dist, world: int, rank: int):
         import ctypes
         import torch
         from . import _abi
         from .qengine import QEngineCUDA
+        self.chunk_floor = self.CHUNK_FLOOR[precision]
         self.torch, self.dist, self.world, self.rank = torch, dist, world, rank
         self.lib = _abi.load()
         self.abi = _abi
@@ -836,9 +840,10 @@ class _ShardedBackend:
             g = ops[j]
             if not g.diag and g.t in far and far[g.t] > horizon:
                 far[g.t] = j
-        # k local logical qubits with the farthest next non-diagonal use (ties: higher physical position = cheaper)
-        lo = self.shard.min_victim_bit
-        cands = [q for q in far if self.perm[q] >= lo] if (nl - lo) >= k else list(far.keys())
+        # k local logical qubits with the farthest next non-diagonal use (ties: higher physical position = cheaper), on
+        # physical bits >= min_victim_bit when the page has k of them, else on any bit >= chunk_floor (never below it)
+        lo = self.shard.min_victim_bit if (nl - self.shard.min_victim_bit) >= k else self.shard.chunk_floor
+        cands = [q for q in far if self.perm[q] >= lo]
         victims = sorted(cands, key=lambda q: (-far[q], -self.perm[q]))[:k]
         if self.shard.needs_top:
             # bring the victims to the top k local positions with local swaps, then exchange bit nl-k+b <-> rank bit b
@@ -889,6 +894,12 @@ class QEngineSharded(QEngineHost):
 
     def _make_backend(self, n_qubits: int):
         k = int(round(math.log2(self._world))) if self._world > 1 else 0
+        floor = P2PShardBuffers.CHUNK_FLOOR[self.precision] if self._p2p else ShardBuffers.chunk_floor
+        if n_qubits - k - floor < k:
+            # an exchange trades the k rank bits for k local qubits on bits >= floor: the page must hold that many
+            raise ValueError("QEngineSharded: %d qubits over %d ranks leave %d local qubits at or above bit %d, fewer than "
+                             "the %d an exchange needs; use fewer ranks or more qubits"
+                             % (n_qubits, self._world, max(n_qubits - k - floor, 0), floor, k))
         if self._p2p:
             shard = P2PShardBuffers(n_qubits - k, self.precision, self._device.index, self._dist, self._world, self._rank)
         else:

@@ -12,6 +12,7 @@ from emu_engine import QEngineEmu
 class EmuP2PShard:
     needs_top = False
     min_victim_bit = 1
+    chunk_floor = 0   # the exchange is a host transposition: any local qubit can trade places with a rank bit
 
     def __init__(self, n_local, precision, dist, world, rank):
         self.nl, self.precision, self.dist, self.world, self.rank = n_local, precision, dist, world, rank

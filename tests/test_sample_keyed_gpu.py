@@ -244,4 +244,4 @@ def test_sharded_sampling_on_gpus(prec, mode, tmp_path):
         except Exception as e:
             if "EADDRINUSE" not in str(e) or attempt == 2:
                 raise
-    scpu.check_ranks_against_oracle([np.load(out + ".%d.npz" % r) for r in range(world)], prec)
+    scpu.check_ranks_against_oracle([np.load(out + ".%d.npz" % r) for r in range(world)], prec, exact=False)

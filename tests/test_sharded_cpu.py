@@ -148,13 +148,17 @@ def test_grover_on_sharded_engine_follows_success_law(tmp_path):
     assert abs(float(gres[0]) - law) < 1e-5
 
 
+# 40 gate layers on 10 qubits, then controls and phases across the rank bits: many exchanges at 4 ranks
+DEEP = qscript.random_htcnot(10, 24, seed=9, timed=False) + qscript.random_u3_cnot(10, 8, seed=5).split("\n", 1)[1]
+DEEP += "CCNOT 9 8 0\nMCPhase 2 9 1 8 0.6 0.8 1 0\nAntiCNOT 8 9\n" + "".join("Prob %d\n" % q for q in range(10))
+
+
 @pytest.mark.parametrize("defer", ["0", "1"])
 def test_deep_circuit_in_order_and_deferred_exchanges(defer, tmp_path, monkeypatch):
     """40 gate layers on 10 qubits over 4 ranks: both exchange policies (in-order, and deferral of the gates blocked by a
     rank-bit target with commutation-aware look-ahead) must reproduce the single-engine oracle."""
     monkeypatch.setenv("B200SV_SHARD_DEFER", defer)
-    text = qscript.random_htcnot(10, 24, seed=9, timed=False) + qscript.random_u3_cnot(10, 8, seed=5).split("\n", 1)[1]
-    text += "CCNOT 9 8 0\nMCPhase 2 9 1 8 0.6 0.8 1 0\nAntiCNOT 8 9\n" + "".join("Prob %d\n" % q for q in range(10))
+    text = DEEP
     want, wres = util.run_engine(text, QEngineRestate, 32)
     got, gres, exchanges = run_sharded(text, 4, 32, tmp_path)
     d = float(np.abs(got.astype(np.complex128) - want[0].astype(np.complex128)).max())

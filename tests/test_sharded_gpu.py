@@ -86,17 +86,43 @@ def _worker_queries(rank, world, port, text, prec, out_path):
         def make(n, perm):
             return QEngineSharded(n, perm, random.Random(1), 1.0 + 0j, precision=prec, dist=dist, world=world, rank=rank,
                                   device=torch.device("cuda", rank), make_engine=cuda_engine_factory(rank, prec), p2p=True)
-        regs, results = qscript.run(text, make)
-        q = regs[0]
-        q.UpdateRunningNorm()
-        nrm = q.GetRunningNorm()
-        perm = q.MAll()                       # on-device sampling across the shards, then collapse
-        amp = q.GetAmplitude(perm)
+        z = queries_26q(make, text)
         if rank == 0:
-            np.savez(out_path, results=np.array([v for _, vals in results for v in vals], dtype=np.float64), norm=nrm, perm=perm,
-                     amp=abs(amp), exchanges=q.be.exchanges)
+            np.savez(out_path, **z)
     finally:
         dist.destroy_process_group()
+
+
+def queries_26q(make, text):
+    """a 26-qubit script of util.sharded_26q_text on a sharded engine from make(n, perm), then the norm and a sharded MAll;
+    what check_26q reads"""
+    regs, results = qscript.run(text, make)
+    q = regs[0]
+    q.UpdateRunningNorm()
+    nrm = q.GetRunningNorm()
+    perm = q.MAll()                       # on-device sampling across the shards, then collapse
+    amp = q.GetAmplitude(perm)
+    return dict(results=np.array([v for _, vals in results for v in vals], dtype=np.float64), norm=nrm, perm=perm,
+                amp=abs(amp), exchanges=q.be.exchanges)
+
+
+def check_26q(z, kind):
+    """queries_26q's results against what the compiled reference QEngineCPU returned (stored results): all per-qubit Prob,
+    48 sampled amplitudes (1e-6), the norm, and a sharded MAll.  Returns the largest amplitude and Prob deviations."""
+    n = 26
+    ref = util.load_reference("sharded_26q_%s" % kind)
+    want = np.array([v for _, vals in ref["results"] for v in vals], dtype=np.float64)
+    # the fp32 reference sums each Prob (2^25 terms) in fp32 per worker thread with a dynamic work split: its own value wanders by
+    # ~1e-4 from run to run.  The per-qubit probabilities are therefore taken from the fp64 build of the reference (same circuit).
+    want_p = np.array([v for _, vals in ref["results64"] for v in vals], dtype=np.float64)[:n]
+    got = z["results"]
+    assert got.shape == want.shape
+    d_amp, d_p = np.abs(got[n:] - want[n:]).max(), np.abs(got[:n] - want_p).max()
+    assert d_amp <= util.AMP_TOL[32], (kind, d_amp)   # amplitudes (re, im pairs): the parity bar
+    # Prob (ours: fp32 state, double accumulation) against the fp64 reference: what is left is the fp32 state's own rounding
+    assert d_p <= 2e-5, (kind, d_p)
+    assert abs(float(z["norm"]) - 1.0) < 1e-4 and float(z["amp"]) > 0.999, kind
+    return float(d_amp), float(d_p)
 
 
 @pytest.mark.parametrize("kind", ["htcnot", "qv", "grover"])
@@ -108,13 +134,7 @@ def test_sharded_26q_against_the_compiled_reference(kind, tmp_path):
     if ng < 2:
         pytest.skip("needs >= 2 GPUs")
     world = 8 if ng >= 8 else (4 if ng >= 4 else 2)
-    n = 26
     text = util.sharded_26q_text(kind)
-    ref = util.load_reference("sharded_26q_%s" % kind)
-    want = np.array([v for _, vals in ref["results"] for v in vals], dtype=np.float64)
-    # the fp32 reference sums each Prob (2^25 terms) in fp32 per worker thread with a dynamic work split: its own value wanders by
-    # ~1e-4 from run to run.  The per-qubit probabilities are therefore taken from the fp64 build of the reference (same circuit).
-    want_p = np.array([v for _, vals in ref["results64"] for v in vals], dtype=np.float64)[:n]
     import torch.multiprocessing as mp
     out = str(tmp_path / "o.npz")
     for attempt in range(3):
@@ -124,10 +144,4 @@ def test_sharded_26q_against_the_compiled_reference(kind, tmp_path):
         except Exception as e:
             if "EADDRINUSE" not in str(e) or attempt == 2:
                 raise
-    z = np.load(out)
-    got = z["results"]
-    assert got.shape == want.shape
-    assert np.abs(got[n:] - want[n:]).max() <= util.AMP_TOL[32], np.abs(got[n:] - want[n:]).max()   # amplitudes (re, im pairs): the parity bar
-    # Prob (ours: fp32 state, double accumulation) against the fp64 reference: what is left is the fp32 state's own rounding
-    assert np.abs(got[:n] - want_p).max() <= 2e-5, np.abs(got[:n] - want_p).max()
-    assert abs(float(z["norm"]) - 1.0) < 1e-4 and float(z["amp"]) > 0.999
+    check_26q(np.load(out), kind)

@@ -115,6 +115,57 @@ def test_pauli_pair_read_only_launches_flush_zero_and_einval(prec):
     assert np.array_equal(p.GetQuantumState(), phi)
 
 
+def run_observables(make, out_file):
+    """the script of tests/test_sharded_observables_cpu.py on a sharded engine from make(n, perm): the pending X gates and
+    the queries, then a non-diagonal gate on a rank-bit qubit, its exchange, and at once a Pauli string with X on a rank
+    bit (in pull mode the partner's page exists only after the partner's pull sweep, which the query's flush and barrier
+    must wait for).  Saves what check_observables reads."""
+    regs, _ = qscript.run(tcpu.CIRCUIT, make)
+    q = regs[0]
+    q.Finish()
+    text = tcpu.query_text(q.be.perm, q.be.nl)
+    gates = "".join(l + "\n" for l in text.splitlines() if l.startswith("X "))
+    queries = "".join(l + "\n" for l in text.splitlines() if not l.startswith("X "))
+    qscript.run("qubits %d\n" % tcpu.N_QUBITS + gates, lambda n, p: q)
+    before, ex0 = q.GetQuantumState(), q.be.exchanges
+    _, results = qscript.run("qubits %d\n" % tcpu.N_QUBITS + queries, lambda n, p: q)
+    same, ex1 = np.array_equal(before, q.GetQuantumState()), q.be.exchanges
+    nl = q.be.nl
+    r0 = [b for b in range(tcpu.N_QUBITS) if q.be.perm[b] >= nl][0]
+    q.H(r0)
+    q.be.flush()
+    rq = [b for b in range(tcpu.N_QUBITS) if q.be.perm[b] >= nl][0]
+    lq = [b for b in range(tcpu.N_QUBITS) if q.be.perm[b] < nl][1]
+    last = q.ExpectationPauliAll([rq, lq], [1, 3])
+    np.savez(out_file, results=np.array([v for _, vals in results for v in vals], dtype=np.float64), same=same,
+             last=last, ex0=ex0, ex1=ex1, ex2=q.be.exchanges, gates=gates, queries=queries,
+             tail="H %d\n" % r0, tailq="ExpectationPauliAll 2 %d %d 1 3\n" % (rq, lq))
+
+
+def check_observables(z, prec, what=""):
+    """every rank returned the same values, left the state alone and exchanged pages only for the tail's gate; the values
+    are the float64 NumPy reference's on the float64 oracle state, within the engine precision's tolerance relative to each
+    query's scale.  Returns the largest |deviation| / scale."""
+    for r in range(len(z)):
+        assert np.array_equal(z[r]["results"], z[0]["results"]) and float(z[r]["last"]) == float(z[0]["last"]), (what, r)
+        assert bool(z[r]["same"]), "%s, rank %d: the queries changed the state" % (what, r)
+        assert int(z[r]["ex1"]) == int(z[r]["ex0"]) and int(z[r]["ex2"]) == int(z[r]["ex1"]) + 1, (what, r)
+    gates = str(z[0]["gates"])
+    want, _ = util.run_engine(tcpu.CIRCUIT + gates, QEngineRestate, 64)
+    ops = [t for _, t in qscript.parse(str(z[0]["queries"]))]
+    assert z[0]["results"].size == len(ops)
+    worst = 0.0
+    for g, t in zip(z[0]["results"], ops):
+        v, scale, _ = no.query_value(want[0], t[0], t[1:])
+        assert abs(g - v) <= tcpu.TOL[prec] * max(scale, 1e-30), (what, t, g, v)
+        worst = max(worst, abs(g - v) / max(scale, 1e-30))
+    want, _ = util.run_engine(tcpu.CIRCUIT + gates + str(z[0]["tail"]), QEngineRestate, 64)
+    t = qscript.parse(str(z[0]["tailq"]))[0][1]
+    v, scale, _ = no.query_value(want[0], t[0], t[1:])
+    assert abs(float(z[0]["last"]) - v) <= tcpu.TOL[prec] * scale, (what, float(z[0]["last"]), v)
+    return max(worst, abs(float(z[0]["last"]) - v) / scale)
+
+
 def _worker(rank, world, port, prec, out_path, mode):
     import torch
     import torch.distributed as dist
@@ -130,28 +181,7 @@ def _worker(rank, world, port, prec, out_path, mode):
             return QEngineSharded(n, perm, random.Random(1), 1.0 + 0j, precision=prec, dist=dist, world=world, rank=rank,
                                   device=torch.device("cuda", rank), make_engine=cuda_engine_factory(rank, prec),
                                   p2p=mode != "nccl")
-        regs, _ = qscript.run(tcpu.CIRCUIT, make)
-        q = regs[0]
-        q.Finish()
-        text = tcpu.query_text(q.be.perm, q.be.nl)
-        gates = "".join(l + "\n" for l in text.splitlines() if l.startswith("X "))
-        queries = "".join(l + "\n" for l in text.splitlines() if not l.startswith("X "))
-        qscript.run("qubits %d\n" % tcpu.N_QUBITS + gates, lambda n, p: q)
-        ex0 = q.be.exchanges
-        _, results = qscript.run("qubits %d\n" % tcpu.N_QUBITS + queries, lambda n, p: q)
-        ex1 = q.be.exchanges
-        # a non-diagonal gate on a rank-bit qubit, its exchange, and at once a Pauli string with X on a rank bit: in pull mode
-        # the partner's page exists only after the partner's pull sweep, which the query's flush and barrier must wait for
-        nl = q.be.nl
-        r0 = [b for b in range(tcpu.N_QUBITS) if q.be.perm[b] >= nl][0]
-        q.H(r0)
-        q.be.flush()
-        rq = [b for b in range(tcpu.N_QUBITS) if q.be.perm[b] >= nl][0]
-        lq = [b for b in range(tcpu.N_QUBITS) if q.be.perm[b] < nl][1]
-        last = q.ExpectationPauliAll([rq, lq], [1, 3])
-        np.savez(out_path + ".%d.npz" % rank, results=np.array([v for _, vals in results for v in vals], dtype=np.float64),
-                 last=last, ex0=ex0, ex1=ex1, ex2=q.be.exchanges, gates=gates, queries=queries,
-                 tail="H %d\n" % r0, tailq="ExpectationPauliAll 2 %d %d 1 3\n" % (rq, lq))
+        run_observables(make, out_path + ".%d.npz" % rank)
     finally:
         dist.destroy_process_group()
 
@@ -171,18 +201,4 @@ def test_sharded_observables_on_gpus_match_the_oracle(prec, mode, tmp_path):
         except Exception as e:
             if "EADDRINUSE" not in str(e) or attempt == 2:
                 raise
-    z = [np.load(out + ".%d.npz" % r) for r in range(world)]
-    for r in range(world):
-        assert np.array_equal(z[r]["results"], z[0]["results"]) and float(z[r]["last"]) == float(z[0]["last"])
-        assert int(z[r]["ex1"]) == int(z[r]["ex0"]) and int(z[r]["ex2"]) == int(z[r]["ex1"]) + 1
-    gates = str(z[0]["gates"])
-    want, _ = util.run_engine(tcpu.CIRCUIT + gates, QEngineRestate, prec)
-    ops = [t for _, t in qscript.parse(str(z[0]["queries"]))]
-    assert z[0]["results"].size == len(ops)
-    for g, t in zip(z[0]["results"], ops):
-        v, scale, _ = no.query_value(want[0], t[0], t[1:])
-        assert abs(g - v) <= tcpu.TOL[prec] * max(scale, 1e-30), (mode, t, g, v)
-    want, _ = util.run_engine(tcpu.CIRCUIT + gates + str(z[0]["tail"]), QEngineRestate, prec)
-    t = qscript.parse(str(z[0]["tailq"]))[0][1]
-    v, scale, _ = no.query_value(want[0], t[0], t[1:])
-    assert abs(float(z[0]["last"]) - v) <= tcpu.TOL[prec] * scale, (mode, float(z[0]["last"]), v)
+    check_observables([np.load(out + ".%d.npz" % r) for r in range(world)], prec, mode)

@@ -167,23 +167,34 @@ def coarse(keys, weights, top=4):
     return out
 
 
-def check_ranks_against_oracle(z, prec):
-    """every rank returned the same samples and left the state and the qubit map alone; sample_many is sample shot for shot;
-    MultiShotMeasureMask is the read-off of sample for the replayed rnds; the histogram follows the oracle's |psi|^2"""
+def check_ranks_against_oracle(z, prec, exact=True):
+    """every rank returned the same samples and left the state and the qubit map alone; sample_many is sample shot for shot
+    (exact), or (pages whose totals come from a reduction that may round differently from one call to the next, as the
+    device's atomic-add norm does) for every rnd but those within 1e-12 of a page boundary; MultiShotMeasureMask is the
+    read-off of sample for the replayed rnds; the state is the float64 oracle's and the histogram follows its |psi|^2.
+    Returns the largest |delta amp| and histogram deviation."""
+    d_amp = d_hist = 0.0
     for name, circ in CIRCUITS.items():
         for r in range(len(z)):
             for k in ("many", "one", "hist_keys", "hist_counts"):
                 assert np.array_equal(z[r][name + "_" + k], z[0][name + "_" + k]), (name, k, r)
-            assert np.array_equal(z[r][name + "_many"], z[r][name + "_one"]), (name, r, z[r][name + "_rnds"])
+            many, one, rnds = z[r][name + "_many"], z[r][name + "_one"], z[r][name + "_rnds"]
+            off = np.flatnonzero(many != one)
+            if not exact and off.size:
+                cum = np.cumsum(z[r][name + "_tots"])
+                assert (np.abs(rnds[off, None] - cum[None, :]).min(axis=1) <= 1e-12).all(), (name, r, rnds[off], cum)
+            else:
+                assert not off.size, (name, r, rnds[off])
             assert bool(z[r][name + "_replay_ok"].all()), (name, r)
             assert bool(z[r][name + "_same"]), "%s, rank %d: sampling changed the state" % (name, r)
             assert int(z[r][name + "_ex1"]) == int(z[r][name + "_ex0"]), "%s, rank %d: sampling exchanged pages" % (name, r)
         assert int(z[0][name + "_ex0"]) >= 1  # the circuit scrambled the qubit map
         assert bool(z[0][name + "_exchanged_first"])  # the first query ran right after an exchange
         assert bin(int(z[0][name + "_xinv"])).count("1") >= 3
-        want, _ = util.run_engine(circ + str(z[0][name + "_gates"]), QEngineRestate, prec)
+        want, _ = util.run_engine(circ + str(z[0][name + "_gates"]), QEngineRestate, 64)
         psi, mine = want[0], z[0][name + "_state"]
         util.assert_states_close({0: mine}, {0: psi}, prec, name)
+        d_amp = max(d_amp, float(np.abs(mine.astype(np.complex128) - psi).max()))
         # every sample has P > 0, and outside the fallback rules of an all-zero page it lies in [0, 2^n)
         p = npref.probs(psi)
         got = z[0][name + "_many"]
@@ -200,6 +211,8 @@ def check_ranks_against_oracle(z, prec):
         assert counts.sum() == SHOTS_HISTOGRAM
         emp = coarse(z[0][name + "_hist_keys"], counts / SHOTS_HISTOGRAM)
         assert np.abs(emp - coarse(key, p)).max() < 0.06, (name, emp, coarse(key, p))
+        d_hist = max(d_hist, float(np.abs(emp - coarse(key, p)).max()))
+    return d_amp, d_hist
 
 
 def walk_loop(tots, rnd):
