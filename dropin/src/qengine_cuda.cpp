@@ -481,7 +481,9 @@ void QEngineCUDA::CUniformParityRZ(const std::vector<bitLenInt>& controls, const
     for (const bitLenInt& c : controls) {
         cm |= pow2Ocl(c);
     }
-    Check(b200sv_uniform_parity_rz(sv, cm, (uint64_t)(bitCapIntOcl)mask, (double)angle));
+    // QEngineCPU's parity runs over an index whose control bits are cleared (state.cpp:1239-1261): a control inside the mask
+    // does not count
+    Check(b200sv_uniform_parity_rz(sv, cm, (uint64_t)(bitCapIntOcl)mask & ~cm, (double)angle));
 }
 
 // ---- probabilities / measurement (reference state.cpp:1751-2107) ---------------------------------------------------

@@ -18,11 +18,12 @@ import ctypes
 import random
 from typing import List, Tuple
 
-from .qengine import QEngineHost
+from .qengine import QEngineHost, lower_two_target
 
 
 class _RecordBackend:
-    """Backend that only records the single-target Apply2x2 forms the dispatch mirror produces."""
+    """Backend that records the single-target Apply2x2 forms the dispatch mirror produces; a two-target form (ISwap, SqrtSwap,
+    FSim, CSwap, ...) is recorded as the three single-target gates of qengine.lower_two_target."""
 
     def __init__(self, n_qubits: int, precision: int):
         self.nq = n_qubits
@@ -43,11 +44,14 @@ class _RecordBackend:
         diff = off1 ^ off2
         if calc_norm or nrm != 1.0:
             raise NotImplementedError("QCircuit: doNormalize bookkeeping cannot be recorded")
-        if not diff or (diff & (diff - 1)):
-            raise NotImplementedError("QCircuit: only single-target gate forms can be recorded (decompose two-target forms)")
         pmask = 0
         for p in pows:
             pmask |= p
+        if bin(diff).count("1") == 2:
+            self.gates += [(o1, o2, pm, tuple(complex(z) for z in m)) for o1, o2, pm, m in lower_two_target(off1, off2, pmask, mtrx)]
+            return None
+        if not diff or (diff & (diff - 1)):
+            raise NotImplementedError("QCircuit: only one- and two-target gate forms can be recorded")
         self.gates.append((off1, off2, pmask, tuple(complex(z) for z in mtrx)))
         return None
 

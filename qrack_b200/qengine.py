@@ -26,6 +26,32 @@ import numpy as np
 
 REAL1_DEFAULT_ARG = -999.0
 
+X_MTRX = (0j, 1 + 0j, 1 + 0j, 0j)
+
+
+def lower_two_target(off1: int, off2: int, pmask: int, mtrx) -> list:
+    """A two-target Apply2x2 form as three single-target ones: [(off1, off2, pmask, mtrx)] for CNOT(p -> q), the gate on p,
+    CNOT(p -> q).
+
+    Apply2x2(off1, off2, m, pows) applies m to the pairs (i | off1, i | off2) over every i with no bit of pows set.  Here
+    off1 ^ off2 = P | Q (targets p < q); the other pows bits C are controls, and off1 & C = off2 & C holds their values.
+    Let c(j) = j ^ Q where bit p of j is set (CNOT p -> q, an exact permutation and its own inverse).  c touches only bits
+    p and q, so c(i | off) = i | c(off), and it flips Q in exactly one of off1, off2 (the one with P set): c(off1) ^ c(off2)
+    = P.  Hence
+        Apply2x2(off1, off2, m, pows) = c . Apply2x2(c(off1), c(off2), m, pows) . c,
+    where the middle form is single-target on p, controlled by C = off1 & C and by q = bit q of c(off1) (q = 1 for the
+    Swap family, whose off1 is P or Q; q = 0 for a |00>, |11> pair), and psi[c(off1)] holds what psi[off1] held.  It
+    applies the same 2x2 to the same pairs."""
+    diff = off1 ^ off2
+    p = (diff & -diff).bit_length() - 1
+    q = diff.bit_length() - 1
+    P, Q = 1 << p, 1 << q
+
+    def c(j):
+        return j ^ Q if j & P else j
+    cnot = (P, P | Q, P | Q, X_MTRX)
+    return [cnot, (c(off1), c(off2), pmask, tuple(mtrx)), cnot]
+
 
 class QEngineHost:
     """Gate dispatch + norm bookkeeping.  Subclasses provide ``self.be`` (backend primitives)."""
@@ -800,7 +826,57 @@ class QEngineHost:
             cm |= 1 << c
         if self.be.is_zero():
             return
-        self.be.uniform_parity_rz(cm, mask, angle)
+        # the reference's parity runs over an index whose control bits par_for_mask has cleared (state.cpp:1239-1261): a
+        # control inside the mask does not count
+        self.be.uniform_parity_rz(cm, mask & ~cm, angle)
+
+    def UniformlyControlledSingleBit(self, controls, qubitIndex: int, mtrxs, mtrxSkipPowers=(), mtrxSkipValueMask: int = 0):
+        """QEngineCPU::UniformlyControlledSingleBit (state.cpp:1094-1198).  `mtrxs` is the table of 2^(len(controls) +
+        len(mtrxSkipPowers)) 2x2 matrices, flat (4 complex per matrix, row-major, as the reference takes it) or one row of 4
+        per matrix.  Each pair of the target takes the entry whose index is the controls' bits (controls[j] -> bit j) with a
+        zero inserted at each skip power, in the order given, and mtrxSkipValueMask ORed in."""
+        if self.be.is_zero():  # CHECK_ZERO_SKIP
+            return
+        controls = [int(c) for c in controls]
+        skips = [int(p) for p in mtrxSkipPowers]
+        size = 1 << (len(controls) + len(skips))
+        table = np.asarray(mtrxs, dtype=np.complex128).reshape(-1, 4)
+        if table.shape[0] < size:
+            raise ValueError("UniformlyControlledSingleBit: the matrix table needs %d entries, got %d" % (size, table.shape[0]))
+        if not controls:
+            return self.Mtrx([complex(z) for z in table[int(mtrxSkipValueMask)]], qubitIndex)
+        if qubitIndex < 0 or qubitIndex >= self.qubitCount:
+            raise ValueError("UniformlyControlledSingleBit qubitIndex is out-of-bounds!")
+        msg = "UniformlyControlledSingleBit control is out-of-bounds!"
+        if len(set(controls)) != len(controls):
+            raise ValueError(msg + " (Found duplicate qubit indices!)")
+        for c in controls:
+            if c < 0 or c >= self.qubitCount:
+                raise ValueError(msg)
+        nrm = self._r(1.0 / math.sqrt(self.runningNorm)) if self.runningNorm > 0 else 1.0
+        if not (self.doNormalize and (1.0 - nrm) > self.FP_NORM_EPSILON):
+            nrm = 1.0
+        # the entries rounded to the engine's complex type, as the reference's complex array holds them
+        table = table[:size].astype(self.cplx).astype(np.complex128)
+        self.be.uniformly_controlled(controls, qubitIndex, table, skips, int(mtrxSkipValueMask), nrm)
+        if self.doNormalize:
+            self.runningNorm = 1.0
+
+    def _uc_rotation(self, controls, qubitIndex: int, angles, rz: bool):  # qinterface/rotational.cpp:130-168
+        mt = []
+        for i in range(1 << len(controls)):
+            a = self._r(angles[i])
+            cs, sn = self._r(math.cos(a / 2)), self._r(math.sin(a / 2))
+            mt.append([complex(cs, -sn), 0j, 0j, complex(cs, sn)] if rz else [complex(cs), complex(-sn), complex(sn), complex(cs)])
+        self.UniformlyControlledSingleBit(controls, qubitIndex, mt)
+
+    def UniformlyControlledRY(self, controls, qubitIndex: int, angles):
+        """RY(angles[k]) on the target for each permutation k of the control bits"""
+        self._uc_rotation(controls, qubitIndex, angles, False)
+
+    def UniformlyControlledRZ(self, controls, qubitIndex: int, angles):
+        """RZ(angles[k]) on the target for each permutation k of the control bits"""
+        self._uc_rotation(controls, qubitIndex, angles, True)
 
     # ---- state management ----------------------------------------------------------------------------------
     def SetPermutation(self, perm: int, phaseFac: Optional[complex] = None):  # state.cpp:228-254
@@ -1708,6 +1784,16 @@ class _CudaBackend:
 
     def uniform_parity_rz(self, cmask, mask, angle):
         self._ck(self.lib.b200sv_uniform_parity_rz(self.h, cmask, mask, angle))
+
+    def uniformly_controlled(self, controls, target, mtrxs, skip_powers, skip_value_mask, nrm):
+        """b200sv_uniformly_controlled; mtrxs = the (2^(controls + skips), 4) complex table"""
+        import ctypes
+        m = np.ascontiguousarray(np.asarray(mtrxs, dtype=np.complex128).reshape(-1)).view(np.float64)
+        c = (ctypes.c_int * max(len(controls), 1))(*controls)
+        s = (ctypes.c_uint64 * max(len(skip_powers), 1))(*skip_powers)
+        self._ck(self.lib.b200sv_uniformly_controlled(self.h, len(controls), c, target,
+                                                      m.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), len(skip_powers), s,
+                                                      skip_value_mask, nrm))
 
     def apply_m(self, mask, result, nrm: complex):
         self._ck(self.lib.b200sv_apply_m(self.h, mask, result, nrm.real, nrm.imag))

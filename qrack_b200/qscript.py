@@ -23,6 +23,10 @@ Grammar (tokens are whitespace separated; ``<m8>`` = 8 reals = 4 complex row-maj
     PhaseRootN n q                CPhaseRootN n c t
     QFT|IQFT start length
     XMask mask   ZMask mask   PhaseParity radians mask   PhaseRootNMask n mask   ZeroPhaseFlip start length
+    UniformParityRZ mask angle    CUniformParityRZ <cs> mask angle
+    UniformlyControlledSingleBit <cs> t <ss> skipValueMask <m8 per table entry>     (<ss> = n skipPower0 .. skipPower{n-1};
+                                  the table has 2^(len(cs) + n) entries)
+    UniformlyControlledRY|UniformlyControlledRZ <cs> t angle0 .. angle{2^len(cs)-1}
     INC|DEC value start length
     SetPermutation perm   ForceM q result   ForceMReg start length result
     NormalizeState   UpdateRunningNorm
@@ -147,6 +151,20 @@ def run(text: str, make_reg: Callable[[int, int], object]) -> Tuple[Dict[int, ob
             q.PhaseParity(float(t[1]), int(t[2]))
         elif op == "PhaseRootNMask":
             q.PhaseRootNMask(int(t[1]), int(t[2]))
+        elif op == "UniformParityRZ":
+            q.UniformParityRZ(int(t[1]), float(t[2]))
+        elif op == "CUniformParityRZ":
+            c, p = _qubits(t, 1)
+            q.CUniformParityRZ(c, int(t[p]), float(t[p + 1]))
+        elif op == "UniformlyControlledSingleBit":
+            c, p = _qubits(t, 1)
+            skips, p2 = _qubits(t, p + 1)
+            v = [float(x) for x in t[p2 + 1:]]
+            q.UniformlyControlledSingleBit(c, int(t[p]), [complex(v[2 * k], v[2 * k + 1]) for k in range(len(v) // 2)], skips,
+                                           int(t[p2]))
+        elif op in ("UniformlyControlledRY", "UniformlyControlledRZ"):
+            c, p = _qubits(t, 1)
+            getattr(q, op)(c, int(t[p]), [float(x) for x in t[p + 1:]])
         elif op in ("INC", "DEC"):
             getattr(q, op)(int(t[1]), int(t[2]), int(t[3]))
         elif op in ("ROL", "ROR"):

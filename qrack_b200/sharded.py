@@ -15,14 +15,18 @@ qubit pairs each page with one partner page, read in place or received into the 
 ``HighestProbAll(n)`` is a per-rank radix select whose ties go to the smaller LOGICAL index, then one ``all_gather`` of every
 rank's best min(n, page) entries and a merge.  ``MultiShotMeasureMask`` over more than 16 qubits samples every shot as
 ``MAll``'s search would: each rank searches its page on the device for the shots that land there, returning logical indices,
-and one ``all_reduce`` of a slot per shot gathers them.
+and one ``all_reduce`` of a slot per shot gathers them.  A two-target gate (ISwap, SqrtSwap, FSim, CSwap, ...) is queued as
+CNOT, a single-target gate, CNOT, so it is scheduled, deferred and fused like any other gate; ``(C)UniformParityRZ`` is a
+per-rank sign of the angle on the local parity kernel; ``UniformlyControlledSingleBit`` turns rank-bit controls into skip
+powers of the local kernel's table and makes a rank-bit target local with the scheduler's exchange.
 
 ``QEngineSharded`` derives from ``QEngineHost`` — the same gate dispatch mirror as ``QEngineCUDA`` — and supplies a
-backend whose primitives are distributed, so the gate-level ``QInterface`` methods (H, T, CNOT, MC/MAC gates, QFT, INC/DEC,
+backend whose primitives are distributed, so the gate-level ``QInterface`` methods (H, T, CNOT, MC/MAC gates, the Swap family,
+FSim, (C)UniformParityRZ, UniformlyControlledSingleBit / RY / RZ, QFT, INC/DEC,
 ZeroPhaseFlip, Prob*, ForceM, M, MAll, MultiShotMeasureMask, HighestProbAll, HighestProbAll(n), ProbMaskAll,
 Expectation/Variance{BitsAll, BitsFactorized, FloatsFactorized, PauliAll}, ExpectationUnitaryAll past 12 qubits, …) work
 unchanged on top of it.  Primitives
-that are not sharded (Compose/Decompose, ForceMParity, UniformParityRZ, SumSqrDiff, the register expectation primitive, the
+that are not sharded (Compose/Decompose, ForceMParity, SumSqrDiff, the register expectation primitive, the
 per-qubit basis sweep behind ExpectationUnitaryAll up to 12 qubits, reduced density matrices, the single-vector top-n
 primitive ``highest_probs``, lossy checkpoints, the native QAlu sweeps, page ops) raise ``NotImplementedError`` identically
 on every rank.  The local engine and the communicator are injected: ``QEngineCUDA`` over a torch CUDA buffer +
@@ -37,7 +41,7 @@ from typing import Callable, List, Optional, Sequence
 
 import numpy as np
 
-from .qengine import QEngineHost, REAL1_DEFAULT_ARG
+from .qengine import QEngineHost, REAL1_DEFAULT_ARG, X_MTRX, lower_two_target
 
 
 def _bits(mask: int):
@@ -248,6 +252,17 @@ def cuda_engine_factory(device_index: int, precision: int = 32):
     return make
 
 
+def _table_index(offset: int, skip_powers) -> int:
+    """UniformlyControlledSingleBit's table index of a control offset: a zero bit inserted at each skip power, in the
+    order given (state.cpp:1130-1137)"""
+    i, hi = 0, offset
+    for p in skip_powers:
+        low = hi & (p - 1)
+        i |= low
+        hi = (hi ^ low) << 1
+    return i | hi
+
+
 class _Gate:
     __slots__ = ("t", "cmask", "cval", "m", "diag")
 
@@ -403,7 +418,13 @@ class _ShardedBackend:
             if xa != xb:                                        # the pending inversions travel with the qubits
                 self.xinv ^= (1 << a) | (1 << b)
             return None
-        raise NotImplementedError("two-target Apply2x2 forms (ISwap/SqrtSwap/CSwap) are not sharded; decompose them")
+        if bin(diff).count("1") == 2:
+            # ISwap, SqrtSwap, FSim, controlled Swap ...: CNOT(p -> q), the gate on p, CNOT(p -> q) (lower_two_target).  Both
+            # are non-diagonal targets, so a rank-bit target costs the one deferred exchange a single-target gate on it costs
+            for o1, o2, pm, m in lower_two_target(off1, off2, pmask, mtrx):
+                self.apply2x2(o1, o2, list(m), [pm], 1.0, thresh, False)
+            return None
+        raise NotImplementedError("Apply2x2 forms with more than two targets are not sharded")
 
     def xmask(self, mask):
         self.xinv ^= mask   # never executed: see __init__
@@ -420,6 +441,65 @@ class _ShardedBackend:
             ang = (radians / 2) if sign < 0 else -(radians / 2)
             ph = complex(math.cos(ang), math.sin(ang))
             self.loc.Mtrx([ph, 0j, 0j, ph], 0)
+
+    def uniform_parity_rz(self, cmask, mask, angle):
+        """(C)UniformParityRZ: odd parity of the logical mask bits gets e^{i angle}, even parity e^{-i angle}, where every
+        control is 1 (state.cpp:1200-1264).  Diagonal, so no exchange: the stored parity is the local bits' parity, this
+        rank's rank-bit parity and the parity of the pending inversions on the mask; each odd one flips the angle's sign.
+        Rank-bit controls select the ranks that run.  The kernel wants every local control's STORED bit to be 1, so a
+        pending inversion on a local control is executed first (a local X) and cleared."""
+        self.flush()
+        for c in _bits(cmask & self.xinv):
+            if self.perm[c] < self.nl:
+                self._local_gate([], 0, list(X_MTRX), self.perm[c])
+                self.xinv ^= 1 << c
+        self._submit_batch()
+        for c in _bits(cmask):
+            pc = self.perm[c]
+            if pc >= self.nl and ((self.rank >> (pc - self.nl)) & 1) == ((self.xinv >> c) & 1):
+                return   # a rank-bit control that is 0 on this rank
+        lc, _ = self._split(self._pmask(cmask))
+        lm, gm = self._split(self._pmask(mask))
+        if (bin(self.rank & gm).count("1") + bin(self.xinv & mask).count("1")) & 1:
+            angle = -angle
+        if lm or lc:
+            self.loc.be.uniform_parity_rz(lc, lm, angle)
+        else:  # no local bit in the mask, no local control: the parity is even on the page, a per-page scalar e^{-i angle}
+            ph = complex(math.cos(angle), -math.sin(angle))
+            self.loc.Mtrx([ph, 0j, 0j, ph], 0)
+
+    def uniformly_controlled(self, controls, target, mtrxs, skip_powers, skip_value_mask, nrm):
+        """UniformlyControlledSingleBit over the pages (state.cpp:1094-1198).  Table index of a pair = the controls' logical
+        bits (controls[j] -> bit j) with zeros inserted at the skip powers, then skip_value_mask ORed in; control j lands on
+        table bit pos[j].  On this rank:
+          * a rank-bit control has one value: it becomes a skip power at pos[j], and its value goes into the skip value mask;
+          * a local control with a pending inversion reads its stored bit flipped: entry e is served from entry e ^ 2^pos[j]
+            (the table is permuted on the host; a position the skip value mask already sets is read as 1 either way);
+          * a pending inversion on the target conjugates every matrix by X.
+        A target on a rank bit is made local first, by the scheduler's exchange."""
+        self.flush()
+        if self.perm[target] >= self.nl:
+            self._exchange([], 0)
+        pos = [_table_index(1 << j, skip_powers).bit_length() - 1 for j in range(len(controls))]
+        lctrls, lpos, flip, svm = [], [], 0, skip_value_mask
+        for j, c in enumerate(controls):
+            x, pc = (self.xinv >> c) & 1, self.perm[c]
+            if pc >= self.nl:
+                if ((self.rank >> (pc - self.nl)) & 1) ^ x:
+                    svm |= 1 << pos[j]
+            else:
+                lctrls.append(pc)
+                lpos.append(pos[j])
+                flip |= x << pos[j]
+        table = np.asarray(mtrxs, dtype=np.complex128).reshape(-1, 4)
+        flip &= ~skip_value_mask
+        if flip:
+            table = table[np.arange(table.shape[0], dtype=np.int64) ^ flip]
+        if (self.xinv >> target) & 1:
+            table = table[:, ::-1]                              # X m X
+        bits = len(controls) + len(skip_powers)
+        skips = [1 << b for b in range(bits) if b not in lpos]  # ascending: the local controls fill the other positions in order
+        self.loc.be.uniformly_controlled(lctrls, self.perm[target], table, skips, svm, nrm)
 
     def phase_root_n_mask(self, n, mask):
         if self.xinv & mask:
@@ -720,7 +800,7 @@ class _ShardedBackend:
             mine = torch.cat(parts, 1).cpu().numpy()
         return merge_top_n(mine[0].view(np.uint64), mine[1].view(np.float64), n)
 
-    _UNSUPPORTED = ("collapse_parity", "uniform_parity_rz", "uniformly_controlled", "inner", "expectation",
+    _UNSUPPORTED = ("collapse_parity", "inner", "expectation",
                     "moments_basis", "reduced_density_matrix", "highest_probs", "lossy_save", "lossy_load",
                     "compose", "decompose", "dispose_perm", "get_page", "set_page", "copy_page", "shuffle", "copy_state", "clone")
 
